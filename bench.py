@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- vehicle-steps/second of the CityFlow step engine on B200 (BASELINE.json metric).
+"""bench.py -- vehicle-steps/second of the CityFlow step engine on an H100 (BASELINE.json metric).
 
 A "step" is one Engine::nextStep over the whole road network.  Workload at N=1: the 30x30 grid of
 BASELINE.json configs[2] with the dense random-walk demand of SURVEY.md Appendix A (frac=0.5, interval=10 s,
@@ -21,6 +21,10 @@ two lane observations), one engine replica per GPU.
 Prints ONE JSON line on rank 0 (task contract): value / e2e / roofline / cpu_baseline / clocks / gpu_launches, plus
 `parity_check`: the sum of get_vehicle_count() over the timed steps of this run next to the same sum taken from the
 compiled reference on the same scenario and the same step window.
+
+`--dump-outputs DIR` writes the public API's view of the state after the last step of the `value` window (lane counts,
+per-vehicle speed and distance, see engine_outputs) as DIR/<name>.npy; the scenario is seeded, so two builds run with the
+same arguments can be compared array for array.
 """
 import argparse
 import importlib.util
@@ -75,9 +79,12 @@ def parse_args():
                    help="N>1, see the module docstring ('sharded' = 'weak')")
     p.add_argument("--clock-ms", type=int, default=50, help="nvidia-smi sampling period (0 = off)")
     p.add_argument("--profile-steps", type=int, default=0,
-                   help="ncu mode: after prefill+warmup run this many steps between cudaProfilerStart/Stop and exit "
-                        "(use with ncu --profile-from-start off)")
+                   help="profiler mode: after prefill+warmup run this many steps between cudaProfilerStart/Stop and exit")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write what the timed path computed in its last timed step to DIR/<name>.npy (see dump_outputs)")
     a = p.parse_args()
+    if a.steps < 1:
+        p.error("--steps must be at least 1")
     if a.multi == "sharded":
         a.multi = "weak"
     if a.lane_change:
@@ -132,8 +139,47 @@ def scaling_of(args):
 
 
 # ----------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def engine_outputs(eng):
+    """What a caller of the public API receives after a step, as arrays in a build-independent order: lanes in the
+    engine's lane order, vehicles sorted by (flow, index) of their id "flow_<f>_<i>"."""
+    import numpy as np
+    lanes = eng.lane_ids()
+    cnt, wait = eng.get_lane_vehicle_count(), eng.get_lane_waiting_vehicle_count()
+    speed, dist = eng.get_vehicle_speed(), eng.get_vehicle_distance()
+    ids = sorted(speed, key=lambda v: tuple(int(x) for x in v.rsplit("_", 2)[-2:]))
+    return {
+        "vehicle_count": np.array([eng.get_vehicle_count()], np.float64),
+        "current_time": np.array([eng.get_current_time()], np.float64),
+        "lane_vehicle_count": np.array([cnt[l] for l in lanes], np.float64),
+        "lane_waiting_vehicle_count": np.array([wait[l] for l in lanes], np.float64),
+        "vehicle_key": np.array([[int(x) for x in v.rsplit("_", 2)[-2:]] for v in ids], np.float64).reshape(-1, 2),
+        "vehicle_speed": np.array([speed[v] for v in ids], np.float64),
+        "vehicle_distance": np.array([dist[v] for v in ids], np.float64),
+    }
+
+
+def dump_outputs(directory, arrays):
+    """DIR/<name>.npy, float64.  Over DUMP_LIMIT_BYTES in all, the per-vehicle arrays are cut to a fixed, seeded sample
+    of rows (the same rows for the same vehicle count)."""
+    import numpy as np
+    limit = DUMP_LIMIT_BYTES - 4096 * len(arrays)   # room for the .npy headers
+    total = sum(a.nbytes for a in arrays.values())
+    if total > limit:
+        n = len(arrays["vehicle_speed"])
+        per_row = sum(a.nbytes for k, a in arrays.items() if k.startswith("vehicle_") and len(a) == n) / max(n, 1)
+        keep = int(max(0, limit - (total - per_row * n)) // per_row)
+        rows = np.sort(np.random.default_rng(0).choice(n, size=min(keep, n), replace=False))
+        arrays = {k: (a[rows] if k.startswith("vehicle_") and len(a) == n else a) for k, a in arrays.items()}
+    os.makedirs(directory, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(directory, k + ".npy"), np.ascontiguousarray(a, np.float64))
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons (B200_PROFILING.md recipe).  Runs for the whole life of the process;
+    """nvidia-smi clocks / throttle reasons.  Runs for the whole life of the process;
     mark() remembers how many samples exist at a moment, so a window of the log can be summarised afterwards."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -194,7 +240,7 @@ def measured_peak_gbs():
         d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json, copy bandwidth)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md, 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not measured)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -348,6 +394,11 @@ def run_ours(args):
     ms_flush_max = reduce_max(ms_flush)
     vs_total = reduce_sum(vs_flush)
     value = vs_total / (ms_flush_max / 1e3)
+    if args.dump_outputs:   # the state after the last step of the `value` window (every rank reads: the getters may be collective)
+        outputs = engine_outputs(eng)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, outputs)
+        barrier()
 
     # same, back to back without flush (state stays L2 resident, as in real stepping); median of chunks so that one
     # host hiccup (the host paces this loop) does not decide the number
@@ -417,17 +468,11 @@ def run_ours(args):
         "k_notify": 16 * n_now + 24 * (n_drv),
         "k_ingest": 12 * n_drv,
     }
-    try:  # DRAM bytes per launch from the committed ncu --set full capture (same workload)
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic_bytes_per_launch.json")))
-    except Exception:
-        traffic = {}
-    same_workload = (args.rows, args.cols, args.frac, args.flow_interval) == (30, 30, 0.5, 10.0)
 
     def roof(k):
         gbs = alg[k] / (kms[k] * 1e-3) / 1e9 if kms[k] > 0 else 0.0
         return {"kernel": k, "bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak,
-                "traffic": traffic.get(k) if same_workload else None,
-                "note": "latency-bound at this size (state is L2-sized; dependent loads + FP64 div/sqrt chains), see profiles/",
+                "note": "latency-bound at this size (state is L2-sized; dependent loads + FP64 div/sqrt chains)",
                 "algorithmic_bytes_per_launch": alg[k], "avg_launch_ms": kms[k], "peak_source": peak_src}
 
     line = None
@@ -543,7 +588,11 @@ def run_ours_rl(args, ranks, sampler):
     inters = rl_intersections(cfg)
     ranks.barrier()
     m_lo = sampler.mark() if rank == 0 else 0
-    r = rl_loop(cityflow, cfg, inters, args.steps, device=local)
+    keep = []
+    r = rl_loop(cityflow, cfg, inters, args.steps, keep=keep, device=local)
+    if args.dump_outputs and rank == 0:   # the state after the last step of the `value` loop
+        dump_outputs(args.dump_outputs, engine_outputs(keep.pop()))
+    keep.clear()
     # the same loop with observations / actions staying on the GPU (cityflow_b200 extras; a stand-in policy of a few torch ops)
     eng = cityflow.Engine(cfg, thread_num=1, device=local)
     for _ in range(100):

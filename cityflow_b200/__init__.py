@@ -1,7 +1,7 @@
-"""cityflow_b200 -- B200-native step engine behind the ``cityflow.Engine`` Python surface.
+"""cityflow_b200 -- H100-native step engine behind the ``cityflow.Engine`` Python surface.
 
 ``Engine`` is the pybind11 class built from ``csrc/pymodule.cpp`` over the C-ABI in
-``include/cityflow_b200.h`` (``libcityflow_b200.so``: host loader + sm_100a kernels).  There is no
+``include/cityflow_b200.h`` (``libcityflow_b200.so``: host loader + sm_90a kernels).  There is no
 CPU fallback: importing works anywhere (so the package can be built and inspected on a CPU box),
 but constructing an ``Engine`` without a CUDA device raises ``RuntimeError``.
 """

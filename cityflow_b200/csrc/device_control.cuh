@@ -11,10 +11,9 @@ namespace cfb {
 // `n.pos` set; `foeLinkW` = linkInfo.w of the notified vehicle's laneLink: turn | type << 8).  Same FP64
 // expressions as the reference, evaluated on the same committed state (nothing between k_notify and k_control
 // changes a vehicle, a blocker or delStep).
-// Measured (profiles/): against the asker doing everything (round 1) k_control 35.0 -> 24.7 us and k_notify 16.9 ->
-// 24.9 us at 1.3e5 vehicles, step 0.0936 -> with PDL 0.0894 ms.  A lighter record (k_notify only gathers the foe's
-// fields, the asker computes the reach steps and walks the blocker chain) was tried too: k_notify 20.5 / k_control 33.2 us,
-// step 0.0963 ms at 1.3e5 vehicles, 2 % faster only at 1.5e6 -- this form stays.
+// Chosen over the asker doing everything (k_control shorter by more than k_notify grows, at 1.3e5 vehicles) and over a
+// lighter record (k_notify only gathers the foe's fields, the asker computes the reach steps and walks the blocker
+// chain), on the GPU the engine was first built for; the split has not been re-measured on the H100.
 __device__ __forceinline__ void foeTerms(const View &V, Notify &n, int foeLinkW) {
     const int fp = n.pos;
     const int4 fid = V.ids[fp];

@@ -2,8 +2,7 @@
 // with -DCFB_CONTROL_COOP; never timed (written when no GPU was left).  Logic verified on the emulated device.
 //
 // Why: k_control lasts as long as its slowest thread, and the slowest threads are the few vehicles that walk
-// four or five flagged crosses one after the other (profiles/r01c_control_cycles.md: 55 k cycles against a mean
-// of 17 k), while most lanes of their warp -- the vehicles further back on the same lane -- have nothing to do
+// four or five flagged crosses one after the other (a per-thread cycle count showed 3x the mean for them), while most lanes of their warp -- the vehicles further back on the same lane -- have nothing to do
 // during that loop.  Here every flagged cross at or beyond a vehicle is a work item in shared memory, the 32
 // lanes evaluate the warp's items side by side (Cross::canPass has no side effect), and each vehicle then takes
 // the first failing cross of its own list in link order.  Same arithmetic, same results; the grid-stride loop is

@@ -2,7 +2,7 @@
 // Engine::scheduleLaneChange / insertShadow (engine.cpp:792-820, lanechange.cpp:71-102), yieldSpeed (:186-206) and the
 // partner coupling of Engine::vehicleControl (engine.cpp:195-244).
 //
-// STATUS: part of the library.  On a B200 it is bit-equal, every field of every vehicle including shadows, every step,
+// STATUS: part of the library.  On the GPU (H100) it is bit-equal, every field of every vehicle including shadows, every step,
 // to the restatement -- which is pinned against oracle/_ref/refdump_lcorder, the reference with its per-worker vehicle
 // sets ordered by priority instead of by heap address (tests/test_gpu_parity.py::test_lane_change_vs_restatement,
 // tools/lc_gpu_check.py; compute-sanitizer racecheck clean) -- and statistically equal to the unmodified reference.

@@ -1,4 +1,4 @@
-// B200 (sm_100a) step engine: device-resident vehicle state + the kernel sequence that replaces
+// H100 (sm_90a) step engine: device-resident vehicle state + the kernel sequence that replaces
 // the reference's barrier-delimited thread phases (Engine::nextStep, engine.cpp:566-594).
 //
 // Data layout (see DESIGN.md §3).  Vehicles do not live in a slot-indexed pool; they live in
@@ -488,7 +488,7 @@ struct DeviceSim::Impl {
     LcCtrl *hLcCtrl = nullptr;        // pinned readback
     int lcSpareCap = 0;
     int slotCap = 0;
-    int numSMs = 148;
+    int numSMs = 132;   // H100 SXM; read from the device at construction
     int gridNotify = 0, gridMove = 0, gridLeader = 0, gridControl = 0;
     bool mirrorStale = false;   // something other than a step changed active / error (reset, restore, a setter): read the device
     bool usePdl = true;   // CITYFLOW_B200_NO_PDL=1: plain stream order between the step kernels
@@ -1339,7 +1339,7 @@ void DeviceSim::ensureGrids() {
 // ---- measurement support: CUDA-event brackets on the engine's own stream ----
 void DeviceSim::flushL2() {
     Impl &I = *impl_;
-    const size_t bytes = (size_t) 256 << 20;  // > 126 MB L2
+    const size_t bytes = (size_t) 256 << 20;  // several times the 50 MB L2 of an H100
     if (I.flushBuf.n < bytes) I.flushBuf.alloc(bytes);
     CFB_CUDA(cudaMemsetAsync(I.flushBuf.p, (int) (steps_ & 0xff), bytes, I.stream));
 }

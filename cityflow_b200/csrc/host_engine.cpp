@@ -358,10 +358,8 @@ public:
     std::unique_ptr<Workers> workers;
     // Used for steps that spawn at least this many vehicles (CITYFLOW_B200_PARALLEL_SPAWN_MIN; 0 = never).  The bench flows
     // spawn in bursts (every flow every 10 s), so this is every tenth step of any bench run: 1 800 creations on one GPU,
-    // 14 400 on every rank of the 8-GPU run (a sharded run replicates the whole network's spawns).  Measured on a B200 host
-    // (4 ranks, 30x120, profiles/r02i): spawn generation 147 -> 95 us per step, end to end 0.260 -> 0.161 ms per step,
-    // parity_check equal; reworked after that (thread-local vectors, one buffer of draws: DESIGN.md section 8), measured in
-    // the kernel-free spawner mode of the test build only: 170 -> 120 us per step at the 8-GPU population.  The RNG, the slot
+    // 14 400 on every rank of the 8-GPU run (a sharded run replicates the whole network's spawns).  The threads split the
+    // creation work only (thread-local vectors, one buffer of draws: DESIGN.md section 8).  The RNG, the slot
     // hand-out and the flow clocks stay sequential.
     int parallelSpawnMin = 512;
     std::vector<int> parSlot, parIndex;
@@ -522,7 +520,7 @@ public:
         // advance because the RNG can be run ahead on a copy: priority, thread index, priority, ... (engine.cpp:601-606).
         // A priority collision makes the real sequence leave the predicted one -- then the remaining prefetches are merely
         // useless.  The prefetches run a fixed distance ahead of the creations: a core tracks only a dozen or so outstanding
-        // line fills, so issuing all of a step's prefetches up front drops most of them (measured: 285 -> see profiles/).
+        // line fills, so issuing all of a step's prefetches up front drops most of them.
         const size_t nDue = due.size();
         constexpr size_t PF = 12;
         const bool parallel = parallelSpawnMin > 0 && nDue >= (size_t) parallelSpawnMin;

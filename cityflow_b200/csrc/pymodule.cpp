@@ -256,7 +256,7 @@ public:
     void loadFromFile(const std::string &path) { check(cfb_load_from_file(e_, path.c_str())); }
     cfb_engine *raw() { return e_; }
     [[noreturn]] void unsupported(const char *what) const {
-        throw std::runtime_error(std::string(what) + " is not implemented by the B200 engine yet");
+        throw std::runtime_error(std::string(what) + " is not implemented by the GPU engine yet");
     }
     // measurement helpers (not part of the reference surface)
     int64_t gpuLaunches() const { return cfb_gpu_launches(e_); }
@@ -303,7 +303,7 @@ Archive::Archive(Engine &e) : a_(cfb_snapshot(e.raw())) {
 }  // namespace
 
 PYBIND11_MODULE(_cityflow_b200, m) {
-    m.doc() = "B200-native CityFlow step engine (drop-in for cityflow.Engine)";
+    m.doc() = "H100-native CityFlow step engine (drop-in for cityflow.Engine)";
     py::class_<Engine>(m, "Engine")
         .def(py::init<const std::string &, int, int, int, int, const py::bytes &>(), "config_file"_a, "thread_num"_a = 1,
              "device"_a = -1, "shard_rank"_a = 0, "shard_world"_a = 1, "nccl_id"_a = py::bytes())

@@ -1,4 +1,4 @@
-/* cityflow_b200 -- C ABI of the B200-native CityFlow step engine.
+/* cityflow_b200 -- C ABI of the H100-native CityFlow step engine.
  *
  * The reference has no C interface: its boundary is the C++ class CityFlow::Engine
  * (src/engine/engine.h:114-183) exposed to Python by pybind11 (src/cityflow.cpp:10-48).  This

@@ -12,7 +12,7 @@ fit: not the 30x30 ones (capacity of the emulated device) and not the device-res
 
 It is NOT a way to run the product on a CPU: nothing in cityflow_b200/ can load these libraries, the emulated device
 refuses to start without CFB_EMULATED_DEVICE_FOR_TESTS=1 (set here), and a run with this plugin says nothing about
-kernels on hardware -- the driver's `pytest -m gpu` on a B200 does not load it."""
+kernels on hardware -- the driver's `pytest -m gpu` on an H100 does not load it."""
 import ctypes
 import os
 import sys

@@ -8,7 +8,6 @@ test_fuzzed_network_vs_compiled_reference, test_vehicle_setters_step_by_step_vs_
    vehicle.cpp:323-329, and so does the engine).
 2. set_vehicle_speed / set_vehicle_route step by step against the restatement (pinned against the reference's Python module
    by tests/test_cpu.py::test_port_oracle_vs_reference_python_api).
-First run on a B200 in round 2: 12 of 12 networks and the API run equal (profiles/r02a_gpu_validation_lc_deadend.log).
 """
 import os
 import sys

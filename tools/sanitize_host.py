@@ -8,7 +8,7 @@ change, a three-rank loop-back group, fuzzed irregular networks, both archive fo
     python tools/sanitize_host.py thread         # -fsanitize=thread, kernel-free spawner mode only (four-thread creation, collisions)
 
 A report aborts the child (non-recoverable); the script prints "clean" when every stage ran.  The GPU-side twin is
-tools/sanitize_run.py (compute-sanitizer on a B200).  TEST INFRASTRUCTURE: the emulated device is not a CPU path of the
+tools/sanitize_run.py (compute-sanitizer on the GPU).  TEST INFRASTRUCTURE: the emulated device is not a CPU path of the
 product (it refuses to start without CFB_EMULATED_DEVICE_FOR_TESTS=1 and nothing in cityflow_b200/ can load it)."""
 import os
 import subprocess
