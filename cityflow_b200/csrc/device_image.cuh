@@ -48,6 +48,52 @@ inline std::vector<std::pair<void *, size_t>> snapshotRegions(const View &V, siz
 constexpr long long IMAGE_MAGIC = 0x43464241LL;
 inline size_t imagePad(size_t b) { return (b + 255) & ~(size_t) 255; }
 
+struct ImageHeader {
+    long long steps = 0;
+    int slotCap = 0;
+    std::vector<size_t> regions;   // bytes of every region
+    size_t bytes() const { return (4 + regions.size()) * sizeof(long long); }
+    size_t payload() const { size_t t = 0; for (size_t b : regions) t += imagePad(b); return t; }
+};
+inline ImageHeader imageHeader(long long steps, int slotCap, const std::vector<std::pair<void *, size_t>> &regs) {
+    ImageHeader h{steps, slotCap, {}};
+    for (auto &r : regs) h.regions.push_back(r.second);
+    return h;
+}
+// out: h.bytes()
+inline void writeImageHeader(const ImageHeader &h, unsigned char *out) {
+    std::vector<long long> w = {IMAGE_MAGIC, h.steps, (long long) h.slotCap, (long long) h.regions.size()};
+    for (size_t b : h.regions) w.push_back((long long) b);
+    memcpy(out, w.data(), w.size() * sizeof(long long));
+}
+// The header of a serialised image of n bytes; throws unless the image is complete.
+inline ImageHeader readImageHeader(const unsigned char *data, size_t n) {
+    if (n < 4 * sizeof(long long)) throw std::runtime_error("cityflow_b200: truncated archive");
+    long long w[4];
+    memcpy(w, data, sizeof w);
+    if (w[0] != IMAGE_MAGIC) throw std::runtime_error("cityflow_b200: not an archive of this engine");
+    ImageHeader h{w[1], (int) w[2], {}};
+    const size_t nr = (size_t) w[3];
+    if (n < (4 + nr) * sizeof(long long)) throw std::runtime_error("cityflow_b200: truncated archive");
+    h.regions.resize(nr);
+    for (size_t k = 0; k < nr; ++k) {
+        long long b;
+        memcpy(&b, data + (4 + k) * sizeof(long long), sizeof b);
+        h.regions[k] = (size_t) b;
+    }
+    if (n < h.bytes() + h.payload()) throw std::runtime_error("cityflow_b200: truncated archive");
+    return h;
+}
+// An image restored into the regions `regs` of an engine (snapshotRegions): the slot-indexed regions may be shorter.
+inline void checkImageFits(const ImageHeader &h, const std::vector<std::pair<void *, size_t>> &regs, const View &V) {
+    if (h.regions.size() != regs.size()) throw std::runtime_error("cityflow_b200: archive does not match this engine");
+    for (size_t k = 0; k < regs.size(); ++k) {
+        if (h.regions[k] > regs[k].second) throw std::runtime_error("cityflow_b200: archive does not match this engine (region size)");
+        if (k + imageSlotRegions(V) < regs.size() && h.regions[k] != regs[k].second)
+            throw std::runtime_error("cityflow_b200: archive was taken on a different road network");
+    }
+}
+
 // A typed window into a serialised image.  The regions start 232 + k * 256 bytes into the buffer (the header is not a
 // multiple of 16 bytes), so the 16-byte-aligned CUDA vector types must not be accessed through pointers of their own type:
 // every access is a memcpy of one element.
@@ -74,26 +120,20 @@ inline std::vector<size_t> imageRegionBytes(const ImageGeometry &G, size_t S) {
 
 // Lay the typed pointers over `blob`; checks the header against this engine's geometry.
 inline ImageArrays imageMap(unsigned char *blob, size_t n, const ImageGeometry &G) {
-    if (n < 4 * sizeof(long long)) throw std::runtime_error("cityflow_b200: truncated archive");
-    long long h[4];
-    memcpy(h, blob, sizeof h);
-    if (h[0] != IMAGE_MAGIC) throw std::runtime_error("cityflow_b200: not an archive of this engine");
+    const ImageHeader h = readImageHeader(blob, n);
     ImageArrays A{};
-    A.steps = h[1];
-    A.slotCap = (int) h[2];
+    A.steps = h.steps;
+    A.slotCap = h.slotCap;
     if (A.slotCap < 0) throw std::runtime_error("cityflow_b200: corrupt archive (slot capacity)");
     const std::vector<size_t> want = imageRegionBytes(G, (size_t) A.slotCap);
-    if ((size_t) h[3] != want.size() || n < (4 + want.size()) * sizeof(long long)) throw std::runtime_error("cityflow_b200: archive does not match this engine");
-    size_t off = (4 + want.size()) * sizeof(long long);
+    if (h.regions.size() != want.size()) throw std::runtime_error("cityflow_b200: archive does not match this engine");
+    size_t off = h.bytes();
     unsigned char *ptr[32];
     for (size_t k = 0; k < want.size(); ++k) {
-        long long have;
-        memcpy(&have, blob + (4 + k) * sizeof(long long), sizeof have);
-        if ((size_t) have != want[k]) throw std::runtime_error("cityflow_b200: archive was taken on a different road network");
+        if (h.regions[k] != want[k]) throw std::runtime_error("cityflow_b200: archive was taken on a different road network");
         ptr[k] = blob + off;
         off += imagePad(want[k]);
     }
-    if (off > n) throw std::runtime_error("cityflow_b200: truncated archive");
     int k = 0;
     A.kin.p = ptr[k++]; A.gap.p = ptr[k++]; A.leader.p = ptr[k++]; A.ids.p = ptr[k++];
     A.nav.p = ptr[k++]; A.cust.p = ptr[k++]; A.count.p = ptr[k++]; A.entCnt.p = ptr[k++];
@@ -154,12 +194,9 @@ inline void encodeImage(const StateImage &in, const ImageGeometry &G, std::vecto
         (int) in.remain.size() != G.nInter)
         throw std::runtime_error("cityflow_b200: archive does not match this road network");
     const size_t S = (size_t) std::max(in.slotCount, 1);
-    const std::vector<size_t> bytes = imageRegionBytes(G, S);
-    std::vector<long long> hdr = {IMAGE_MAGIC, in.step, (long long) S, (long long) bytes.size()};
-    size_t total = 0;
-    for (size_t b : bytes) { hdr.push_back((long long) b); total += imagePad(b); }
-    blob.assign(hdr.size() * sizeof(long long) + total, 0);
-    memcpy(blob.data(), hdr.data(), hdr.size() * sizeof(long long));
+    const ImageHeader h{in.step, (int) S, imageRegionBytes(G, S)};
+    blob.assign(h.bytes() + h.payload(), 0);
+    writeImageHeader(h, blob.data());
     const ImageArrays A = imageMap(blob.data(), blob.size(), G);
     const int par = (int) (in.step & 1);
     for (size_t p = 0; p < G.P; ++p) { A.leader.set(p, -1); A.cust.set(p, NAN); }

@@ -62,9 +62,7 @@ namespace cg = cooperative_groups;
 }  // namespace cfb
 #include "device_view.cuh"
 #include "device_image.cuh"
-namespace cfb {
-
-}  // namespace cfb
+#include "device_layout.cuh"
 #include "device_phases_a.cuh"
 namespace cfb {
 // Programmatic dependent launch: the five step kernels are chained with programmatic stream serialisation, so the next
@@ -83,14 +81,7 @@ __global__ void __launch_bounds__(256) k_notify(View V) { pdlEnter(); phase_noti
 #include "device_control.cuh"
 namespace cfb {
 
-#ifdef CFB_CONTROL_COOP
-}  // namespace cfb
-#include "device_control_coop.cuh"   // EXPERIMENT: the warp evaluates its vehicles' crosses side by side
-namespace cfb {
-__global__ void __launch_bounds__(256, 4) k_control(View V) { pdlEnter(); phase_control_coop(V, blockIdx.x, gridDim.x); }
-#else
 __global__ void __launch_bounds__(256, 4) k_control(View V) { pdlEnter(); phase_control(V, blockIdx.x, gridDim.x); }
-#endif
 
 }  // namespace cfb
 #include "device_phases_b.cuh"
@@ -343,6 +334,9 @@ struct DevBuf {
 // memsets, device-to-device copies, staged pageable uploads).  Every function that writes device
 // state that way ends with this barrier, before anything can be enqueued on the engine's stream.
 static void legacySync() { CFB_CUDA(cudaStreamSynchronize(cudaStreamLegacy)); }
+static void applyFills(const std::vector<Fill> &fills) {
+    for (const Fill &f : fills) if (f.bytes) CFB_CUDA(cudaMemset(f.p, f.byte, f.bytes));
+}
 
 // A step kernel, optionally with programmatic stream serialisation (see pdlEnter()).
 template <class... A>
@@ -359,32 +353,18 @@ static void launchPdl(void (*k)(A...), int grid, int block, cudaStream_t s, bool
     cfg.numAttrs = pdl ? 1 : 0;
     CFB_CUDA(cudaLaunchKernelEx(&cfg, k, args...));
 }
-static void launchStepKernel(void (*k)(View), int grid, int block, cudaStream_t s, bool pdl, const View &V) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = pdl ? 1 : 0;
-    CFB_CUDA(cudaLaunchKernelEx(&cfg, k, V));
-}
 
 struct DeviceSim::Impl {
     DeviceSimOptions opt;
     View V{};
     cudaStream_t stream = nullptr;
     int P = 0;
-    std::vector<int> offHost;
-    std::vector<double> phase0Time;   // remainDuration after TrafficLight::init(0)
+    DeviceLayout L;                   // host copy of the static tables (device_layout.cuh)
     // static
     DevBuf<double> drvLength, drvMaxSpeed, lcDist, phaseTime;
     DevBuf<int> off, laneOutBeg, laneOutLinks, llStartLane, llEndLane, llRoadLink, llCrossBeg, lcIdx, csLink,
         interPhaseBeg, interRLBeg, phaseAvailBeg, rlInter, planBeg, planData;
-    DevBuf<unsigned char> llTurn, llType, phaseAvail, interVirtual;
+    DevBuf<unsigned char> phaseAvail, interVirtual;
     DevBuf<DTmpl> tmpl;
     // dynamic
     DevBuf<double2> kin, nkin, mkin;
@@ -394,7 +374,6 @@ struct DeviceSim::Impl {
     DevBuf<int> act0, act1, extra, lcPeer, blk, delStep, boundOut, boundIn;
     DevBuf<unsigned char> owned;
     DevBuf<int> ingBuf;
-    std::vector<int> ingLists;
     DevBuf<TailMsg> tailSend, tailRecv;
     DevBuf<MoverMsg> moverSend, moverRecv;
     DevBuf<int2> blkUpd, blkAll;
@@ -520,24 +499,6 @@ struct DeviceSim::Impl {
     }
 };
 
-static DTmpl toDevice(const VehicleTemplate &t, double interval) {
-    DTmpl d{};
-    d.len = t.len;
-    d.maxPosAcc = t.maxPosAcc;
-    d.maxNegAcc = t.maxNegAcc;
-    d.usualPosAcc = t.usualPosAcc;
-    d.usualNegAcc = t.usualNegAcc;
-    d.minGap = t.minGap;
-    d.maxSpeed = t.maxSpeed;
-    d.headwayTime = t.headwayTime;
-    d.yieldDistance = t.yieldDistance;
-    d.turnSpeed = t.turnSpeed;
-    // vehicle.cpp:42-44 (and the identical look-ahead bound at :190-191)
-    d.approachDist = t.maxSpeed * t.maxSpeed / t.usualNegAcc / 2 + t.maxSpeed * interval * 2;
-    d.speed0 = t.speed;
-    return d;
-}
-
 DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &templates, const Routing &routing,
                      const DeviceSimOptions &opt)
     : impl_(new Impl()) {
@@ -564,87 +525,27 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
         if (!coop) I.useCoop = false;
     }
     View &V = I.V;
-    const int nL = net.nLanes(), nK = net.nLinks(), nD = nL + nK;
-    V.nLanes = nL; V.nLinks = nK; V.nDrv = nD; V.nInter = net.nInter(); V.nRL = net.nRoadLinks(); V.nCross = net.nCross();
     V.dt = opt.interval;
     V.rl = opt.rlTrafficLight ? 1 : 0;
 
     // ---- static tables ----
-    std::vector<double> len(nD), maxs(nD);
-    std::vector<int> off(nD + 1, 0);
-    for (int d = 0; d < nD; ++d) {
-        len[d] = d < nL ? net.laneLength[d] : net.llLength[d - nL];
-        maxs[d] = d < nL ? net.laneMaxSpeed[d] : 10000.0;  // LaneLink::maxSpeed, roadnet.h:456
-        // bucket capacity: room for bumper-to-bumper traffic of 2.5 m vehicles plus slack
-        int cap = (int) (len[d] / 2.5) + 8;
-        cap = (cap + 3) & ~3;
-        off[d + 1] = off[d] + cap;
-    }
-    I.P = off[nD];
-    I.offHost = off;
-    I.drvLength.upload(len); I.drvMaxSpeed.upload(maxs); I.off.upload(off);
-    std::vector<int> lob(nL + 1, 0), lol;
-    for (int l = 0; l < nL; ++l) {
-        for (int ll : net.laneOutLinks[l]) lol.push_back(ll);
-        lob[l + 1] = (int) lol.size();
-    }
-    if (lol.empty()) lol.push_back(0);
-    I.laneOutBeg.upload(lob); I.laneOutLinks.upload(lol);
-    std::vector<unsigned char> turn(std::max(nK, 1)), type(std::max(nK, 1));
-    std::vector<int> lcb(nK + 1, 0), lcIdx, csLink(std::max(2 * net.nCross(), 1), 0), llRL(net.llRoadLink);
-    std::vector<double> lcDist;
-    for (int k = 0; k < nK; ++k) {
-        turn[k] = net.linkIsTurn(k) ? 1 : 0;
-        type[k] = (unsigned char) net.rlType[net.llRoadLink[k]];
-        for (const CrossRef &c : net.llCrosses[k]) {
-            lcIdx.push_back(c.cross * 2 + c.side);
-            lcDist.push_back(net.crossDist[c.side][c.cross]);
-        }
-        lcb[k + 1] = (int) lcIdx.size();
-    }
-    for (int c = 0; c < net.nCross(); ++c) {
-        csLink[2 * c] = net.crossLink[0][c];
-        csLink[2 * c + 1] = net.crossLink[1][c];
-    }
-    // peer index: where the same cross sits in the crossing link's list; mask width
-    std::vector<int> lcPeer(lcIdx.size(), 0), flatOf(std::max(2 * net.nCross(), 1), 0);
-    int maxCross = 1;
-    for (int k = 0; k < nK; ++k) {
-        maxCross = std::max(maxCross, lcb[k + 1] - lcb[k]);
-        for (int q = lcb[k]; q < lcb[k + 1]; ++q) flatOf[lcIdx[q]] = q;
-    }
-    for (size_t q = 0; q < lcIdx.size(); ++q) lcPeer[q] = flatOf[lcIdx[q] ^ 1];
-    V.maskWords = (maxCross + 31) / 32;
-    if (lcIdx.empty()) { lcIdx.push_back(0); lcDist.push_back(0); lcPeer.push_back(0); }
-    I.lcPeer.upload(lcPeer);
-    V.lcPeer = I.lcPeer.p;
-    auto nz = [](std::vector<int> v) { if (v.empty()) v.push_back(0); return v; };
-    I.llStartLane.upload(nz(net.llStartLane)); I.llEndLane.upload(nz(net.llEndLane)); I.llRoadLink.upload(nz(llRL));
-    I.llTurn.upload(turn); I.llType.upload(type);
-    {
-        std::vector<int4> li(std::max(nK, 1), make_int4(0, 0, 0, 0));
-        for (int k = 0; k < nK; ++k) li[k] = make_int4(net.llRoadLink[k], net.llEndLane[k], lcb[k], (int) turn[k] | ((int) type[k] << 8));
-        I.linkInfo.upload(li);
-        V.linkInfo = I.linkInfo.p;
-    }
-    I.llCrossBeg.upload(lcb); I.lcIdx.upload(lcIdx); I.lcDist.upload(lcDist); I.csLink.upload(csLink);
-    I.interPhaseBeg.upload(net.interPhaseBeg); I.interRLBeg.upload(net.interRoadLinkBeg);
-    I.phaseAvailBeg.upload(nz(net.phaseAvailBeg)); I.rlInter.upload(nz(net.rlInter));
-    std::vector<double> pt = net.phaseTime; if (pt.empty()) pt.push_back(0);
-    I.phaseTime.upload(pt);
-    std::vector<unsigned char> pa = net.phaseAvail; if (pa.empty()) pa.push_back(0);
-    I.phaseAvail.upload(pa);
-    std::vector<unsigned char> iv(net.interVirtual.begin(), net.interVirtual.end());
-    I.interVirtual.upload(iv);
-    I.phase0Time.assign(net.nInter(), 0.0);
-    for (int i = 0; i < net.nInter(); ++i)
-        if (!net.interVirtual[i]) I.phase0Time[i] = net.phaseTime[net.interPhaseBeg[i]];
+    I.L = deviceLayout(net, V);
+    const DeviceLayout &L = I.L;
+    const int nL = V.nLanes, nK = V.nLinks, nD = V.nDrv;
+    I.P = L.P;
+    I.drvLength.upload(L.drvLength); I.drvMaxSpeed.upload(L.drvMaxSpeed); I.off.upload(L.off);
+    I.laneOutBeg.upload(L.laneOutBeg); I.laneOutLinks.upload(L.laneOutLinks);
+    I.llStartLane.upload(L.llStartLane); I.llEndLane.upload(L.llEndLane); I.llRoadLink.upload(L.llRoadLink);
+    I.linkInfo.upload(L.linkInfo);
+    I.llCrossBeg.upload(L.llCrossBeg); I.lcIdx.upload(L.lcIdx); I.lcDist.upload(L.lcDist); I.lcPeer.upload(L.lcPeer); I.csLink.upload(L.csLink);
+    I.interPhaseBeg.upload(L.interPhaseBeg); I.interRLBeg.upload(L.interRLBeg);
+    I.phaseAvailBeg.upload(L.phaseAvailBeg); I.rlInter.upload(L.rlInter);
+    I.phaseTime.upload(L.phaseTime); I.phaseAvail.upload(L.phaseAvail); I.interVirtual.upload(L.interVirtual);
 
     V.drvLength = I.drvLength.p; V.drvMaxSpeed = I.drvMaxSpeed.p; V.off = I.off.p;
     V.laneOutBeg = I.laneOutBeg.p; V.laneOutLinks = I.laneOutLinks.p;
-    V.llStartLane = I.llStartLane.p; V.llEndLane = I.llEndLane.p; V.llRoadLink = I.llRoadLink.p;
-    V.llTurn = I.llTurn.p; V.llType = I.llType.p;
-    V.llCrossBeg = I.llCrossBeg.p; V.lcIdx = I.lcIdx.p; V.lcDist = I.lcDist.p; V.csLink = I.csLink.p;
+    V.llStartLane = I.llStartLane.p; V.llEndLane = I.llEndLane.p; V.llRoadLink = I.llRoadLink.p; V.linkInfo = I.linkInfo.p;
+    V.llCrossBeg = I.llCrossBeg.p; V.lcIdx = I.lcIdx.p; V.lcDist = I.lcDist.p; V.lcPeer = I.lcPeer.p; V.csLink = I.csLink.p;
     V.interPhaseBeg = I.interPhaseBeg.p; V.interRLBeg = I.interRLBeg.p; V.phaseAvailBeg = I.phaseAvailBeg.p;
     V.rlInter = I.rlInter.p; V.phaseTime = I.phaseTime.p; V.phaseAvail = I.phaseAvail.p; V.interVirtual = I.interVirtual.p;
 
@@ -658,20 +559,17 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
     I.waitHead.alloc(std::max(nL, 1)); I.waitTail.alloc(std::max(nL, 1)); I.inserted.alloc(std::max(nL, 1));
     I.notify.alloc(std::max(2 * net.nCross(), 1));
     I.curPhase.alloc(net.nInter()); I.remain.alloc(net.nInter()); I.rlAvail.alloc(std::max(net.nRoadLinks(), 1));
-    V.moverCap = (int) std::min<size_t>(P, (size_t) 1 << 22);
     I.mkin.alloc(V.moverCap); I.mids.alloc(V.moverCap); I.mnav.alloc(V.moverCap);
-    I.cust.alloc(P); I.cust.fill(0xff); V.cust = I.cust.p;
+    I.cust.alloc(P); V.cust = I.cust.p;
     I.tail.alloc(nD); I.foeMask.alloc((size_t) std::max(nK, 1) * V.maskWords);
     V.tail = I.tail.p; V.foeMask = I.foeMask.p;
 #ifdef CFB_DEBUG_COUNTERS
     I.dbgCyc.alloc(P); I.dbgPath.alloc(P); I.dbgCyc.fill(0); I.dbgPath.fill(0);
     V.dbgCyc = I.dbgCyc.p; V.dbgPath = I.dbgPath.p;
 #endif
-    V.vehCap = I.P;
     I.vehList0.alloc(P); I.vehList1.alloc(P); I.act0.alloc(nD); I.act1.alloc(nD); I.extra.alloc(nD);
     V.vehList[0] = I.vehList0.p; V.vehList[1] = I.vehList1.p; V.actList[0] = I.act0.p; V.actList[1] = I.act1.p;
     V.extraList = I.extra.p;
-    V.finCap = 1 << 20;
     I.finSlots.alloc(V.finCap);
     I.ctrl.alloc(1);
     CFB_CUDA(cudaMallocHost(&I.hCtrl, sizeof(Ctrl)));
@@ -739,12 +637,10 @@ void DeviceSim::uploadTemplates(const std::vector<VehicleTemplate> &templates) {
 
 void DeviceSim::uploadPlans(const Routing &routing) {
     Impl &I = *impl_;
-    std::vector<int> pb = routing.planBeg(), pd = routing.planData();
-    if (pb.empty()) pb.push_back(0);
-    if (pd.empty()) pd.push_back(PLAN_END);
+    const PlanTables T = planTables(routing);
     CFB_CUDA(cudaStreamSynchronize(I.stream));
-    I.planBeg.upload(pb);
-    I.planData.upload(pd);
+    I.planBeg.upload(T.planBeg);
+    I.planData.upload(T.planData);
     I.V.planBeg = I.planBeg.p;
     I.V.planData = I.planData.p;
     I.graphDirty = true;
@@ -799,25 +695,11 @@ void DeviceSim::ensureSlotCapacity(int slots) {
 void DeviceSim::reset() {
     Impl &I = *impl_;
     CFB_CUDA(cudaStreamSynchronize(I.stream));
-    I.count.fill(0); I.entCnt.fill(0);
-    I.waitHead.fill(0xff); I.waitTail.fill(0xff); I.inserted.fill(0);
-    I.pos.fill(0xff); I.waitNext.fill(0xff); I.cust.fill(0xff); I.slotCust.fill(0xff);
-    I.blk.fill(0xff); I.delStep.fill(0x80);
-    if (I.arena.p) CFB_CUDA(cudaMemset(I.V.delStep, 0x80, (size_t) Impl::SHARD_SLOT_CAP * sizeof(int)));   // (lives in the arena)
-    I.notify.fill(0);
-    I.tail.fill(0xff);   // pos = -1: every drivable empty
-    I.foeMask.fill(0);
-    I.curPhase.fill(0);
+    applyFills(resetFills(I.V, (size_t) I.P, (size_t) I.slotCap));
+    CFB_CUDA(cudaMemcpy(I.remain.p, I.L.remain0.data(), I.L.remain0.size() * sizeof(double), cudaMemcpyHostToDevice));
     I.hPhase.assign(I.V.nInter, 0);
     I.phaseDirty = false;
     I.hPhaseStale = false;
-    CFB_CUDA(cudaMemcpy(I.remain.p, I.phase0Time.data(), I.phase0Time.size() * sizeof(double), cudaMemcpyHostToDevice));
-    I.rlAvail.fill(0);
-    int epoch = 0;   // the seam messages of a sharded run are stamped with it: it never goes back
-    CFB_CUDA(cudaMemcpy(&epoch, &I.V.ctrl->epoch, sizeof(int), cudaMemcpyDeviceToHost));
-    I.ctrl.fill(0);
-    legacySync();
-    CFB_CUDA(cudaMemcpy(&I.V.ctrl->epoch, &epoch, sizeof(int), cudaMemcpyHostToDevice));
     if (I.hMirror) { I.hMirror[1] = 0; I.hMirror[2] = 0; I.hMirror[3] = 0; }   // (the stream is idle: nothing else writes it now)
     I.mirrorStale = false;
     // leader = -1 everywhere is not required (only occupied positions are read)
@@ -876,15 +758,15 @@ void DeviceSim::step(const SpawnRec *recs, int n) {
     auto launchAll = [&](bool withEvents) {
         const bool pdl = I.usePdl && !withEvents;   // (events between the kernels would serialise them anyway)
         if (withEvents) cudaEventRecord(I.ev[0], s);
-        launchStepKernel(k_ingest, std::max(gLaneRL, 1), TPB, s, false, V);   // follows a copy, not a kernel
+        launchPdl(k_ingest, std::max(gLaneRL, 1), TPB, s, false, V);   // follows a copy, not a kernel
         if (withEvents) cudaEventRecord(I.ev[1], s);
-        launchStepKernel(k_notify, I.gridNotify, TPB, s, pdl, V);
+        launchPdl(k_notify, I.gridNotify, TPB, s, pdl, V);
         if (withEvents) cudaEventRecord(I.ev[2], s);
-        launchStepKernel(k_control, I.gridControl, 256, s, pdl, V);
+        launchPdl(k_control, I.gridControl, 256, s, pdl, V);
         if (withEvents) cudaEventRecord(I.ev[3], s);
-        launchStepKernel(k_move, I.gridMove, TPB, s, pdl, V);
+        launchPdl(k_move, I.gridMove, TPB, s, pdl, V);
         if (withEvents) cudaEventRecord(I.ev[4], s);
-        launchStepKernel(k_leader, I.gridLeader, TPB, s, pdl, V);
+        launchPdl(k_leader, I.gridLeader, TPB, s, pdl, V);
         if (withEvents) cudaEventRecord(I.ev[5], s);
     };
     if (!tm && I.useCoop) {
@@ -966,43 +848,16 @@ void DeviceSim::configureShard(int rank, int world, const std::vector<unsigned c
     I.shardRank = rank;
     I.shardWorld = world;
     I.bsize = boundarySize;
-    std::vector<unsigned char> own3 = owned;
-    for (int q = 0; q < world; ++q)
-        for (int l : feedPerPeer[q]) own3[l] = 2;   // ghost lanes: admitted into locally, never listed as work
-    I.owned.upload(own3);
+    const ShardLists SL = shardLists(V.nLanes, V.nLinks, owned, feedPerPeer, ownPerPeer, ownedRoadLinks);
+    I.owned.upload(SL.owned);
     I.ownedHost = owned;
     V.owned = I.owned.p;
-    {   // k_ingest walks these instead of every lane / laneLink / roadLink of the whole network
-        std::vector<int> lanes, links, rls;
-        for (int l = 0; l < V.nLanes; ++l) if (own3[l]) lanes.push_back(l);
-        for (int k = 0; k < V.nLinks; ++k) if (owned[V.nLanes + k]) links.push_back(k);
-        for (int r = 0; r < (int) ownedRoadLinks.size(); ++r) if (ownedRoadLinks[r]) rls.push_back(r);
-        V.nIngLanes = (int) lanes.size(); V.nIngLinks = (int) links.size(); V.nIngRL = (int) rls.size();
-        I.ingLists.clear();
-        I.ingLists.insert(I.ingLists.end(), lanes.begin(), lanes.end());
-        I.ingLists.insert(I.ingLists.end(), links.begin(), links.end());
-        I.ingLists.insert(I.ingLists.end(), rls.begin(), rls.end());
-        I.ingLists.push_back(0);
-        I.ingBuf.upload(I.ingLists);
-        V.ingLanes = I.ingBuf.p; V.ingLinks = I.ingBuf.p + lanes.size(); V.ingRL = I.ingBuf.p + lanes.size() + links.size();
-    }
-    std::vector<int> out, in;
-    I.outBeg.assign(1, 0);
-    I.inBeg.assign(1, 0);
-    for (int q = 0; q < world; ++q) {
-        out.insert(out.end(), feedPerPeer[q].begin(), feedPerPeer[q].end());
-        in.insert(in.end(), ownPerPeer[q].begin(), ownPerPeer[q].end());
-        I.outBeg.push_back((int) out.size());
-        I.inBeg.push_back((int) in.size());
-    }
-    V.nBoundOut = (int) out.size();
-    V.nBoundIn = (int) in.size();
-    if (out.empty()) out.push_back(0);
-    if (in.empty()) in.push_back(0);
-    I.boundOut.upload(out);
-    I.boundIn.upload(in);
-    V.boundOut = I.boundOut.p;
-    V.boundIn = I.boundIn.p;
+    I.ingBuf.upload(SL.ing);
+    I.boundOut.upload(SL.boundOut);
+    I.boundIn.upload(SL.boundIn);
+    SL.point(V, I.ingBuf.p, I.boundOut.p, I.boundIn.p);
+    I.outBeg = SL.outBeg;
+    I.inBeg = SL.inBeg;
     I.tailSend.alloc(std::max(V.nBoundIn, 1));
     I.tailRecv.alloc(std::max(V.nBoundOut, 1));
     I.moverSend.alloc(std::max(V.nBoundOut, 1));
@@ -1045,20 +900,20 @@ void DeviceSim::runIngest() {
 void DeviceSim::runNotifyControl() {
     Impl &I = *impl_;
     ensureGrids();
-    launchStepKernel(k_notify, I.gridNotify, 256, I.stream, I.usePdl && !I.timing, I.V);   // behind k_ingest
-    launchStepKernel(k_control, I.gridControl, 256, I.stream, I.usePdl && !I.timing, I.V);
+    launchPdl(k_notify, I.gridNotify, 256, I.stream, I.usePdl && !I.timing, I.V);   // behind k_ingest
+    launchPdl(k_control, I.gridControl, 256, I.stream, I.usePdl && !I.timing, I.V);
     launches_ += 2;
 }
 void DeviceSim::runMove() {
     Impl &I = *impl_;
     ensureGrids();
-    launchStepKernel(k_move, I.gridMove, 256, I.stream, I.usePdl && !I.timing, I.V);
+    launchPdl(k_move, I.gridMove, 256, I.stream, I.usePdl && !I.timing, I.V);
     launches_ += 1;
 }
 void DeviceSim::runLeader() {
     Impl &I = *impl_;
     ensureGrids();
-    launchStepKernel(k_leader, I.gridLeader, 256, I.stream, I.usePdl && !I.timing, I.V);
+    launchPdl(k_leader, I.gridLeader, 256, I.stream, I.usePdl && !I.timing, I.V);
     launches_ += 1;
 }
 void DeviceSim::packTails() {
@@ -1138,24 +993,14 @@ void DeviceSim::shardConnect(const std::vector<void *> &peerBase) {
     I.peers.upload(peers);
     // index tables: where my messages land in the receivers' mailboxes (partition.h)
     const SeamTables T = seamTables(I.bsize, me);
-    const std::vector<int> &nbr = T.nbr, &outPeer = T.outPeer, &outDst = T.outDst, &inPeer = T.inPeer, &inDst = T.inDst;
-    if ((int) outPeer.size() != V.nBoundOut || (int) inPeer.size() != V.nBoundIn) throw std::runtime_error("shardConnect: boundary tables disagree");
-    if ((int) nbr.size() > 120) throw std::runtime_error("shardConnect: too many neighbour ranks");
-    std::vector<int> all;
-    const size_t oN = 0, oOP = oN + nbr.size(), oOD = oOP + outPeer.size(), oIP = oOD + outDst.size(), oID = oIP + inPeer.size(), oT = oID + inDst.size();
-    all.insert(all.end(), nbr.begin(), nbr.end());
-    all.insert(all.end(), outPeer.begin(), outPeer.end());
-    all.insert(all.end(), outDst.begin(), outDst.end());
-    all.insert(all.end(), inPeer.begin(), inPeer.end());
-    all.insert(all.end(), inDst.begin(), inDst.end());
-    all.push_back(0); all.push_back(0);
-    I.p2pInts.upload(all);
+    if ((int) T.outPeer.size() != V.nBoundOut || (int) T.inPeer.size() != V.nBoundIn) throw std::runtime_error("shardConnect: boundary tables disagree");
+    if ((int) T.nbr.size() > 120) throw std::runtime_error("shardConnect: too many neighbour ranks");
+    const SeamIndex X = seamIndex(T);
+    I.p2pInts.upload(X.ints);
     const Impl::ArenaLayout L = Impl::arenaLayout(W, V.nBoundIn, V.nBoundOut);
     ShardP2P &S = I.S;
     S.peers = I.peers.p; S.me = me; S.world = W;
-    S.nbr = I.p2pInts.p + oN; S.nNbr = (int) nbr.size();
-    S.outPeer = I.p2pInts.p + oOP; S.outDst = I.p2pInts.p + oOD; S.inPeer = I.p2pInts.p + oIP; S.inDst = I.p2pInts.p + oID;
-    S.ticket = I.p2pInts.p + oT;
+    X.point(S, I.p2pInts.p);
     S.flags = (int *) (I.arena.p + L.flags);
     S.blkIn = (int2 *) (I.arena.p + L.blkIn);
     S.moverIn = (MoverMsg *) (I.arena.p + L.moverIn);
@@ -1599,55 +1444,48 @@ void DeviceSim::laneVehicleSlots(std::vector<int32_t> &slots, std::vector<int32_
     launches_ += 1;
 }
 
-void DeviceSim::debugDump(std::vector<DebugRec> &out) {
-    Impl &I = *impl_;
+// The arrays the debug records are assembled from (device_layout.cuh), copied to the host.
+struct HostDump {
+    std::vector<int> count, leader, del;
+    std::vector<double2> kin;
+    std::vector<double> gap;
+    std::vector<int4> ids, nav;
+    std::vector<LcSlot> lc;
+    View V{};
+};
+template <class T> static void copyDown(std::vector<T> &dst, const T *src, size_t n) {
+    dst.resize(n);
+    if (n) CFB_CUDA(cudaMemcpy(dst.data(), src, n * sizeof(T), cudaMemcpyDeviceToHost));
+}
+static void dumpToHost(DeviceSim::Impl &I, HostDump &h, bool withLc) {
     CFB_CUDA(cudaStreamSynchronize(I.stream));
     const size_t P = (size_t) I.P;
-    std::vector<int> count(I.V.nDrv), leader(P);
-    std::vector<double2> kin(P);
-    std::vector<double> gap(P);
-    std::vector<int4> ids(P), nav(P);
-    std::vector<int> del(I.slotCap);
-    CFB_CUDA(cudaMemcpy(del.data(), I.V.delStep, del.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    copyDown(h.del, I.V.delStep, (size_t) I.slotCap);
     readCtrlImpl(I.stream, I.hCtrl, I.V.ctrl);
-    const int lastStep = I.hCtrl->step - 1;
-    CFB_CUDA(cudaMemcpy(count.data(), I.V.count, count.size() * sizeof(int), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(leader.data(), I.V.leader, P * sizeof(int), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(kin.data(), I.V.kin, P * sizeof(double2), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(gap.data(), I.V.gap, P * sizeof(double), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(ids.data(), I.V.ids, P * sizeof(int4), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(nav.data(), I.V.nav, P * sizeof(int4), cudaMemcpyDeviceToHost));
-    out.clear();
-    for (int d = 0; d < I.V.nDrv; ++d) {
-        if (!I.ownedHost.empty() && !I.ownedHost[d]) continue;   // sharded: another rank's drivable (only ghost data here)
-        for (int k = 0; k < count[d]; ++k) {
-            const int p = I.offHost[d] + k;
-            DebugRec r{};
-            r.slot = ids[p].x;
-            r.drivable = d;
-            r.leaderSlot = leader[p] >= 0 ? ids[leader[p]].x : -1;
-            r.blockerSlot = nav[p].z;
-            if (r.blockerSlot >= 0 && del[r.blockerSlot] == lastStep) r.blockerSlot = -1;  // dropped lazily on the device
-            r.priority = ids[p].z;
-            r.enterLaneLinkTime = nav[p].w;
-            r.listIndex = k;
-            r.dis = kin[p].x;
-            r.speed = kin[p].y;
-            r.gap = leader[p] >= 0 ? gap[p] : 0.0;
-            out.push_back(r);
-        }
-    }
+    copyDown(h.count, I.V.count, (size_t) I.V.nDrv);
+    copyDown(h.leader, I.V.leader, P);
+    copyDown(h.kin, I.V.kin, P);
+    copyDown(h.ids, I.V.ids, P);
+    copyDown(h.nav, I.V.nav, P);
+    if (withLc) copyDown(h.lc, I.lcSlot.p, (size_t) I.slotCap);
+    else copyDown(h.gap, I.V.gap, P);
+    View &V = h.V;
+    V.nDrv = I.V.nDrv;
+    V.off = I.L.off.data(); V.count = h.count.data(); V.leader = h.leader.data(); V.kin = h.kin.data(); V.gap = h.gap.data();
+    V.ids = h.ids.data(); V.nav = h.nav.data(); V.delStep = h.del.data(); V.ctrl = I.hCtrl; V.lc.slot = h.lc.data();
+}
+
+void DeviceSim::debugDump(std::vector<DebugRec> &out) {
+    HostDump h;
+    dumpToHost(*impl_, h, false);
+    debugRecords(h.V, impl_->ownedHost.empty() ? nullptr : impl_->ownedHost.data(), out);
 }
 
 // ---- snapshot / restore of the whole dynamic state (Archive, archive.cpp:9-151) ----
 // The image stays in device memory (a D2D copy at HBM speed); toHost()/fromHost() serialise it.
 struct DeviceSim::Snapshot {
-    struct Region { size_t bytes; };
-    std::vector<Region> regions;
+    ImageHeader h;
     DevBuf<unsigned char> blob;
-    long long steps = 0;
-    int slotCap = 0;
-    size_t total = 0;
 };
 
 static std::vector<std::pair<void *, size_t>> snapshotRegions(DeviceSim::Impl &I) {   // device_image.cuh
@@ -1664,35 +1502,30 @@ DeviceSim::Snapshot *DeviceSim::snapshot() {
     }
     auto regs = snapshotRegions(I);
     Snapshot *s = new Snapshot();
-    for (auto &r : regs) { s->regions.push_back({r.second}); s->total += (r.second + 255) & ~(size_t) 255; }
-    s->blob.alloc(s->total);
+    s->h = imageHeader(steps_, I.slotCap, regs);
+    s->blob.alloc(s->h.payload());
     size_t off = 0;
     for (auto &r : regs) {
         if (r.second) CFB_CUDA(cudaMemcpyAsync(s->blob.p + off, r.first, r.second, cudaMemcpyDeviceToDevice, I.stream));
-        off += (r.second + 255) & ~(size_t) 255;
+        off += imagePad(r.second);
     }
     CFB_CUDA(cudaStreamSynchronize(I.stream));
-    s->steps = steps_;
-    s->slotCap = I.slotCap;
     return s;
 }
 
 void DeviceSim::restore(const Snapshot *s) {
     Impl &I = *impl_;
-    ensureSlotCapacity(s->slotCap);
+    ensureSlotCapacity(s->h.slotCap);
     CFB_CUDA(cudaStreamSynchronize(I.stream));
     auto regs = snapshotRegions(I);
-    if (regs.size() != s->regions.size()) throw std::runtime_error("cityflow_b200: archive does not match this engine");
-    // slots beyond the archive's capacity: unused
-    I.pos.fill(0xff); I.waitNext.fill(0xff); I.slotCust.fill(0xff); I.blk.fill(0xff); I.delStep.fill(0x80);
+    checkImageFits(s->h, regs, I.V);
+    applyFills(slotFills(I.V, (size_t) I.slotCap));   // slots beyond the archive's capacity: unused
     legacySync();   // the fills land before the image is copied over them on the engine's stream
     size_t off = 0;
     for (size_t k = 0; k < regs.size(); ++k) {
-        const size_t bytes = s->regions[k].bytes;
-        if (bytes > regs[k].second) throw std::runtime_error("cityflow_b200: archive does not match this engine (region size)");
-        if (k + imageSlotRegions(I.V) < regs.size() && bytes != regs[k].second) throw std::runtime_error("cityflow_b200: archive was taken on a different road network");
+        const size_t bytes = s->h.regions[k];
         if (bytes) CFB_CUDA(cudaMemcpyAsync(regs[k].first, s->blob.p + off, bytes, cudaMemcpyDeviceToDevice, I.stream));
-        off += (bytes + 255) & ~(size_t) 255;
+        off += imagePad(bytes);
     }
     I.hPhase.resize(I.V.nInter);
     if (I.V.nInter) {  // on the engine's stream: it is non-blocking, a plain cudaMemcpy would not wait for the copies above
@@ -1707,18 +1540,17 @@ void DeviceSim::restore(const Snapshot *s) {
         if (I.hMirror) { I.hMirror[1] = I.hCtrl->active; I.hMirror[2] = I.hCtrl->error; I.hMirror[3] = I.hCtrl->ties; I.hMirror[0] = I.hCtrl->epoch; }
         I.mirrorStale = false;
     }
-    I.notify.fill(0);      // epoch-stamped scratch: nothing of an older timeline may match
-    I.foeMask.fill(0);
+    applyFills(scratchFills(I.V));
     CFB_CUDA(cudaStreamSynchronize(I.stream));
     legacySync();
-    steps_ = s->steps;
+    steps_ = s->h.steps;
 }
 
 void DeviceSim::freeSnapshot(Snapshot *s) { delete s; }
 
 // The image in decoded form (device_image.cuh): the reference-schema JSON archive of host_engine.cpp goes through these.
 static ImageGeometry imageGeometry(DeviceSim::Impl &I) {
-    return ImageGeometry{I.offHost.data(), I.V.nDrv, I.V.nLanes, I.V.nInter, (size_t) I.P};
+    return ImageGeometry{I.L.off.data(), I.V.nDrv, I.V.nLanes, I.V.nInter, (size_t) I.P};
 }
 void DeviceSim::decodeSnapshot(const Snapshot *s, StateImage &out) {
     std::vector<unsigned char> blob;
@@ -1732,28 +1564,16 @@ DeviceSim::Snapshot *DeviceSim::encodeSnapshot(const StateImage &in) {
 }
 
 void DeviceSim::snapshotToHost(const Snapshot *s, std::vector<unsigned char> &out) {
-    // header: magic, steps, slotCap, #regions, region sizes; then the blob
-    std::vector<long long> hdr = {0x43464241LL, s->steps, (long long) s->slotCap, (long long) s->regions.size()};
-    for (auto &r : s->regions) hdr.push_back((long long) r.bytes);
-    out.resize(hdr.size() * sizeof(long long) + s->total);
-    memcpy(out.data(), hdr.data(), hdr.size() * sizeof(long long));
-    if (s->total) CFB_CUDA(cudaMemcpy(out.data() + hdr.size() * sizeof(long long), s->blob.p, s->total, cudaMemcpyDeviceToHost));
+    out.resize(s->h.bytes() + s->h.payload());
+    writeImageHeader(s->h, out.data());
+    if (s->h.payload()) CFB_CUDA(cudaMemcpy(out.data() + s->h.bytes(), s->blob.p, s->h.payload(), cudaMemcpyDeviceToHost));
 }
 
 DeviceSim::Snapshot *DeviceSim::snapshotFromHost(const unsigned char *data, size_t n) {
-    if (n < 4 * sizeof(long long)) throw std::runtime_error("cityflow_b200: truncated archive");
-    const long long *h = reinterpret_cast<const long long *>(data);
-    if (h[0] != 0x43464241LL) throw std::runtime_error("cityflow_b200: not an archive of this engine");
     Snapshot *s = new Snapshot();
-    s->steps = h[1];
-    s->slotCap = (int) h[2];
-    const size_t nr = (size_t) h[3];
-    if (n < (4 + nr) * sizeof(long long)) { delete s; throw std::runtime_error("cityflow_b200: truncated archive"); }
-    for (size_t k = 0; k < nr; ++k) { s->regions.push_back({(size_t) h[4 + k]}); s->total += ((size_t) h[4 + k] + 255) & ~(size_t) 255; }
-    const size_t hb = (4 + nr) * sizeof(long long);
-    if (n < hb + s->total) { delete s; throw std::runtime_error("cityflow_b200: truncated archive"); }
-    s->blob.alloc(s->total);
-    if (s->total) CFB_CUDA(cudaMemcpy(s->blob.p, data + hb, s->total, cudaMemcpyHostToDevice));
+    s->h = readImageHeader(data, n);
+    s->blob.alloc(s->h.payload());
+    if (s->h.payload()) CFB_CUDA(cudaMemcpy(s->blob.p, data + s->h.bytes(), s->h.payload(), cudaMemcpyHostToDevice));
     legacySync();
     return s;
 }
@@ -1784,7 +1604,7 @@ bool DeviceSim::vehicleState(int slot, VehState &out) {
     CFB_CUDA(cudaMemcpy(&nv, I.V.nav + p, sizeof(nv), cudaMemcpyDeviceToHost));
     if (idv.x != slot) return false;
     out.pos = p;
-    out.drivable = (int) (std::upper_bound(I.offHost.begin(), I.offHost.end(), p) - I.offHost.begin()) - 1;
+    out.drivable = I.L.posDrv[p];
     out.planIdx = nv.x;
     out.nextDrv = idv.w;
     out.dis = k.x;
@@ -1842,17 +1662,9 @@ void DeviceSim::setPhase(int intersection, int phase) {
 void DeviceSim::uploadLanePlans(const Routing &routing) {
     Impl &I = *impl_;
     CFB_CUDA(cudaStreamSynchronize(I.stream));
-    auto up = [](DevBuf<int> &b, std::vector<int> v) { if (v.empty()) v.push_back(0); b.upload(v); };
-    up(I.lcPlanRoute, routing.planRouteTable());
-    up(I.lcPlanRoadPos, routing.planRoadPosTable());
-    up(I.lcLanePlanRoad, routing.lanePlanRoadTable());
-    up(I.lcLanePlanBeg, routing.lanePlanBegTable());
-    up(I.lcLanePlanId, routing.lanePlanIdTable());
-    {
-        std::vector<int> last(std::max(routing.numRoutes(), 1), -1);
-        for (int r = 0; r < routing.numRoutes(); ++r) if (routing.route(r).valid) last[r] = routing.route(r).roads.back();
-        I.lcRouteLastRoad.upload(last);
-    }
+    const LanePlanTables T = lanePlanTables(routing);
+    I.lcPlanRoute.upload(T.planRoute); I.lcPlanRoadPos.upload(T.planRoadPos); I.lcLanePlanRoad.upload(T.lanePlanRoad);
+    I.lcLanePlanBeg.upload(T.lanePlanBeg); I.lcLanePlanId.upload(T.lanePlanId); I.lcRouteLastRoad.upload(T.routeLastRoad);
     LcView &C = I.V.lc;
     C.planRoute = I.lcPlanRoute.p; C.planRoadPos = I.lcPlanRoadPos.p;
     C.lanePlanRoad = I.lcLanePlanRoad.p; C.lanePlanBeg = I.lcLanePlanBeg.p; C.lanePlanId = I.lcLanePlanId.p;
@@ -1860,38 +1672,13 @@ void DeviceSim::uploadLanePlans(const Routing &routing) {
     legacySync();
 }
 
-void DeviceSim::enableLaneChange(const RoadNet &net, const Routing &routing) {
+void DeviceSim::enableLaneChange(const RoadNet &, const Routing &routing) {
     Impl &I = *impl_;
     View &V = I.V;
     CFB_CUDA(cudaStreamSynchronize(I.stream));
-    const int nL = net.nLanes();
-    // Road::buildSegmentationByInterval roadnet.cpp:687-691 with (len + minGap) * MAX_NUM_CARS_ON_SEGMENT of a
-    // default VehicleInfo = (5 + 2) * 10 (roadnet.cpp:305-312, config.h:5); Lane::buildSegmentation :852-861
-    std::vector<int> segBeg(nL + 1, 0), laneIdx(nL), laneRoadN(nL);
-    std::vector<double> segStart, laneWidth(nL);
-    for (int r = 0; r < net.nRoads(); ++r) {
-        double len = 0.0;
-        const auto &pts = net.roadPoints[r];
-        for (size_t i = 0; i + 1 < pts.size(); ++i) {
-            const double dx = pts[i + 1].x - pts[i].x, dy = pts[i + 1].y - pts[i].y;
-            len += sqrt(dx * dx + dy * dy);
-        }
-        const size_t numSegs = std::max((size_t) ceil(len / ((5.0 + 2.0) * 10)), (size_t) 1);
-        for (int l = net.roadLaneBeg[r]; l < net.roadLaneBeg[r + 1]; ++l) {
-            segBeg[l] = (int) segStart.size();
-            for (size_t i = 0; i < numSegs; ++i) segStart.push_back(i * net.laneLength[l] / numSegs);
-            laneIdx[l] = net.laneIdx[l];
-            laneRoadN[l] = net.roadNumLanes(r);
-            laneWidth[l] = net.laneWidth[l];
-        }
-    }
-    segBeg[nL] = (int) segStart.size();
-    std::vector<int> posDrv(I.P);
-    for (int d = 0; d < V.nDrv; ++d)
-        for (int p = I.offHost[d]; p < I.offHost[d + 1]; ++p) posDrv[p] = d;
-    I.lcSegBeg.upload(segBeg); I.lcSegStart.upload(segStart); I.lcLaneIdx.upload(laneIdx); I.lcLaneRoadN.upload(laneRoadN);
-    I.lcLaneWidth.upload(laneWidth); I.lcPosDrv.upload(posDrv);
-    I.lcLaneRoad.upload(net.laneRoad);
+    const DeviceLayout &L = I.L;
+    I.lcSegBeg.upload(L.segBeg); I.lcSegStart.upload(L.segStart); I.lcLaneIdx.upload(L.laneIdx); I.lcLaneRoadN.upload(L.laneRoadN);
+    I.lcLaneWidth.upload(L.laneWidth); I.lcPosDrv.upload(L.posDrv); I.lcLaneRoad.upload(L.laneRoad);
     V.lc.laneRoad = I.lcLaneRoad.p;
     I.lcSegIdx.alloc(I.P); I.lcSegIdx.fill(0);
     I.lcCand.alloc(LC_MAX_CAND); I.lcInvolved.alloc(LC_MAX_CAND); I.lcShadowLog.alloc(LC_MAX_CAND); I.lcPrio.alloc(LC_MAX_CAND);
@@ -1984,39 +1771,9 @@ void DeviceSim::stepLcEnd(const int32_t *priorities, int n) {
 }
 
 void DeviceSim::debugDumpLc(std::vector<LcDebugRec> &out) {
-    Impl &I = *impl_;
-    CFB_CUDA(cudaStreamSynchronize(I.stream));
-    const size_t P = (size_t) I.P;
-    std::vector<int> count(I.V.nDrv), leader(P);
-    std::vector<double2> kin(P);
-    std::vector<int4> ids(P), nav(P);
-    std::vector<LcSlot> lc(I.slotCap);
-    std::vector<int> del(I.slotCap);
-    CFB_CUDA(cudaMemcpy(del.data(), I.V.delStep, del.size() * sizeof(int), cudaMemcpyDeviceToHost));
-    readCtrlImpl(I.stream, I.hCtrl, I.V.ctrl);
-    const int lastStep = I.hCtrl->step - 1;
-    CFB_CUDA(cudaMemcpy(count.data(), I.V.count, count.size() * sizeof(int), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(leader.data(), I.V.leader, P * sizeof(int), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(kin.data(), I.V.kin, P * sizeof(double2), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(ids.data(), I.V.ids, P * sizeof(int4), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(nav.data(), I.V.nav, P * sizeof(int4), cudaMemcpyDeviceToHost));
-    CFB_CUDA(cudaMemcpy(lc.data(), I.lcSlot.p, lc.size() * sizeof(LcSlot), cudaMemcpyDeviceToHost));
-    out.clear();
-    for (int d = 0; d < I.V.nDrv; ++d)
-        for (int k = 0; k < count[d]; ++k) {
-            const int p = I.offHost[d] + k;
-            const LcSlot &L = lc[ids[p].x];
-            LcDebugRec r{};
-            r.slot = ids[p].x; r.priority = ids[p].z; r.partnerType = L.type; r.partnerSlot = L.partner; r.drivable = d;
-            r.leaderSlot = leader[p] >= 0 ? ids[leader[p]].x : -1;
-            r.blockerSlot = nav[p].z;
-            if (r.blockerSlot >= 0 && del[r.blockerSlot] == lastStep) r.blockerSlot = -1;   // dropped lazily on the device
-            r.flags = L.changing | (L.finished << 1);
-            r.lastDir = L.lastDir;
-            r.dis = kin[p].x; r.speed = kin[p].y; r.gap = leader[p] >= 0 ? L.gap : 0.0;
-            r.offset = L.offset; r.waiting = L.waiting; r.lastChange = L.lastChange;
-            out.push_back(r);
-        }
+    HostDump h;
+    dumpToHost(*impl_, h, true);
+    lcDebugRecords(h.V, out);
 }
 
 }  // namespace cfb

@@ -74,7 +74,6 @@ struct View {
     const int *off;
     const int *laneOutBeg, *laneOutLinks;
     const int *llStartLane, *llEndLane, *llRoadLink;
-    const unsigned char *llTurn, *llType;
     const int4 *linkInfo;   // per laneLink {roadLink, endLane, crossBeg, turn | type << 8}
     const int *llCrossBeg, *lcIdx;
     const double *lcDist;

@@ -1,5 +1,5 @@
-// device_hostsim.h -- DeviceSim's arrays on the host + the kernel bodies compiled for the emulated warp
-// (tests/device_emu.h).  TEST INFRASTRUCTURE ONLY: shared by tests/device_step_probe.cpp (emulated engine vs
+// device_hostsim.h -- DeviceSim's arrays on the host (tables from csrc/device_layout.cuh) + the kernel bodies compiled
+// for the emulated warp (tests/device_emu.h).  TEST INFRASTRUCTURE ONLY: shared by tests/device_step_probe.cpp (emulated engine vs
 // the restatement) and tests/device_sim_emu.cpp (the real host engine / C-ABI on top of the emulated device).
 #pragma once
 #include <algorithm>
@@ -18,13 +18,10 @@ namespace cfb { namespace cg = cooperative_groups; }
 #include "device_sim.h"
 #include "device_view.cuh"
 #include "device_phases_a.cuh"
-#include "device_control.cuh"
-#ifdef CFB_CONTROL_COOP
-#include "device_control_coop.cuh"
-#define phase_control phase_control_coop   // the probes then run the cooperative variant as k_control's body
-#endif   // (+ device_lc.cuh, kernels included: blockIdx / gridDim are globals here)
+#include "device_control.cuh"   // (+ device_lc.cuh, kernels included: blockIdx / gridDim are globals here)
 #include "device_phases_b.cuh"
 #include "device_shard.cuh"      // the seam protocol's kernel bodies (peer-memory form), run on the emulated warp too
+#include "device_layout.cuh"
 
 
 namespace cfbtest {
@@ -33,18 +30,19 @@ using namespace cfb;
 
 template <class T> struct Buf : std::vector<T> { T *p() { return this->data(); } };
 
-struct HostSim {   // DeviceSim's arrays (device_sim.cu constructor), on the host
+struct HostSim {   // DeviceSim's arrays on the host: the static tables of device_layout.cuh, the dynamic state allocated here
     View V{};
+    DeviceLayout L;
+    PlanTables plans;
+    LanePlanTables lanePlans;
     int P = 0, slotCap = 0;
-    Buf<double> drvLength, drvMaxSpeed, lcDist, phaseTime, gap, remain, cust, slotCust, segStart, laneWidth;
-    Buf<int> off, laneOutBeg, laneOutLinks, llStartLane, llEndLane, llRoadLink, llCrossBeg, lcIdx, csLink, lcPeer, interPhaseBeg,
-        interRLBeg, phaseAvailBeg, rlInter, planBeg, planData, leader, count, pos, waitHead, waitTail, waitNext, curPhase, entCnt, ent,
-        act0, act1, extra, blk, delStep, segIdx, posDrv, segBeg, laneIdx, laneRoadN, planRoute, planRoadPos, lpRoad, lpBeg, lpId, cand,
-        involved, spare, prio, routeLast, laneRoadT, scratch;
-    Buf<unsigned char> phaseAvail, interVirtual, inserted, rlAvail;
+    Buf<double> gap, remain, cust, slotCust;
+    Buf<int> leader, count, pos, waitHead, waitTail, waitNext, curPhase, entCnt, ent, act0, act1, extra, blk, delStep, segIdx, cand,
+        involved, spare, prio, scratch;
+    Buf<unsigned char> inserted, rlAvail;
     Buf<DTmpl> tmpl;
     Buf<double2> kin, nkin, mkin;
-    Buf<int4> ids, nav, slotInfo, mids, mnav, linkInfo;
+    Buf<int4> ids, nav, slotInfo, mids, mnav;
     Buf<int2> nbuf, finSlots, veh0, veh1, shadowLog;
     Buf<Notify> notify;
     Buf<Tail> tail;
@@ -55,89 +53,34 @@ struct HostSim {   // DeviceSim's arrays (device_sim.cu constructor), on the hos
     LcCtrl lcCtrl{};
     long long steps = 0;
 
-    void init(const RoadNet &net, double interval, bool rl, bool laneChange, const std::vector<std::vector<double>> &segStartPerLane) {
-        const int nL = net.nLanes(), nK = net.nLinks(), nD = nL + nK;
-        V.nLanes = nL; V.nLinks = nK; V.nDrv = nD; V.nInter = net.nInter(); V.nRL = net.nRoadLinks(); V.nCross = net.nCross();
+    void init(const RoadNet &net, double interval, bool rl, bool laneChange) {
+        L = deviceLayout(net, V);
+        const int nL = V.nLanes, nK = V.nLinks, nD = V.nDrv;
         V.dt = interval; V.rl = rl ? 1 : 0;
-        drvLength.resize(nD); drvMaxSpeed.resize(nD); off.assign(nD + 1, 0);
-        for (int d = 0; d < nD; ++d) {
-            drvLength[d] = d < nL ? net.laneLength[d] : net.llLength[d - nL];
-            drvMaxSpeed[d] = d < nL ? net.laneMaxSpeed[d] : 10000.0;
-            int cap = (int) (drvLength[d] / 2.5) + 8;
-            cap = (cap + 3) & ~3;
-            off[d + 1] = off[d] + cap;
-        }
-        P = off[nD];
-        laneOutBeg.assign(nL + 1, 0);
-        for (int l = 0; l < nL; ++l) { for (int ll : net.laneOutLinks[l]) laneOutLinks.push_back(ll); laneOutBeg[l + 1] = (int) laneOutLinks.size(); }
-        if (laneOutLinks.empty()) laneOutLinks.push_back(0);
-        llCrossBeg.assign(nK + 1, 0);
-        for (int k = 0; k < nK; ++k) {
-            for (const CrossRef &c : net.llCrosses[k]) { lcIdx.push_back(c.cross * 2 + c.side); lcDist.push_back(net.crossDist[c.side][c.cross]); }
-            llCrossBeg[k + 1] = (int) lcIdx.size();
-        }
-        csLink.assign(std::max(2 * net.nCross(), 1), 0);
-        for (int c = 0; c < net.nCross(); ++c) { csLink[2 * c] = net.crossLink[0][c]; csLink[2 * c + 1] = net.crossLink[1][c]; }
-        lcPeer.assign(lcIdx.size(), 0);
-        std::vector<int> flatOf(std::max(2 * net.nCross(), 1), 0);
-        int maxCross = 1;
-        for (int k = 0; k < nK; ++k) {
-            maxCross = std::max(maxCross, llCrossBeg[k + 1] - llCrossBeg[k]);
-            for (int q = llCrossBeg[k]; q < llCrossBeg[k + 1]; ++q) flatOf[lcIdx[q]] = q;
-        }
-        for (size_t q = 0; q < lcIdx.size(); ++q) lcPeer[q] = flatOf[lcIdx[q] ^ 1];
-        V.maskWords = (maxCross + 31) / 32;
-        if (lcIdx.empty()) { lcIdx.push_back(0); lcDist.push_back(0); lcPeer.push_back(0); }
-        auto cp = [](Buf<int> &b, const std::vector<int> &v) { b.assign(v.begin(), v.end()); if (b.empty()) b.push_back(0); };
-        cp(llStartLane, net.llStartLane); cp(llEndLane, net.llEndLane); cp(llRoadLink, net.llRoadLink);
-        linkInfo.assign(std::max(nK, 1), make_int4(0, 0, 0, 0));
-        for (int k = 0; k < nK; ++k)
-            linkInfo[k] = make_int4(net.llRoadLink[k], net.llEndLane[k], llCrossBeg[k], (net.linkIsTurn(k) ? 1 : 0) | (net.rlType[net.llRoadLink[k]] << 8));
-        cp(interPhaseBeg, net.interPhaseBeg); cp(interRLBeg, net.interRoadLinkBeg); cp(phaseAvailBeg, net.phaseAvailBeg); cp(rlInter, net.rlInter);
-        phaseTime.assign(net.phaseTime.begin(), net.phaseTime.end()); if (phaseTime.empty()) phaseTime.push_back(0);
-        phaseAvail.assign(net.phaseAvail.begin(), net.phaseAvail.end()); if (phaseAvail.empty()) phaseAvail.push_back(0);
-        interVirtual.assign(net.interVirtual.begin(), net.interVirtual.end());
-        // dynamic
-        kin.assign(P, make_double2(0, 0)); nkin.assign(P, make_double2(0, 0)); gap.assign(P, 0); leader.assign(P, -1);
-        ids.assign(P, make_int4(0, 0, 0, 0)); nav.assign(P, make_int4(0, 0, 0, 0)); nbuf.assign(P, make_int2(0, 0));
-        count.assign(nD, 0); entCnt.assign(nD, 0); ent.assign((size_t) nD * ENT_CAP, 0);
-        waitHead.assign(std::max(nL, 1), -1); waitTail.assign(std::max(nL, 1), -1); inserted.assign(std::max(nL, 1), 0);
-        notify.assign(std::max(2 * net.nCross(), 1), Notify{0.0, 0, 0});
-        curPhase.assign(net.nInter(), 0); remain.assign(net.nInter(), 0.0); rlAvail.assign(std::max(net.nRoadLinks(), 1), 0);
-        for (int i = 0; i < net.nInter(); ++i) if (!net.interVirtual[i]) remain[i] = net.phaseTime[net.interPhaseBeg[i]];
-        V.moverCap = P;
-        mkin.assign(P, make_double2(0, 0)); mids.assign(P, make_int4(0, 0, 0, 0)); mnav.assign(P, make_int4(0, 0, 0, 0));
-        cust.assign(P, NAN);
-        Tail empty{}; empty.pos = -1; empty.prev = -1;
-        tail.assign(nD, empty);
-        foeMask.assign((size_t) std::max(nK, 1) * V.maskWords, 0u);
-        V.vehCap = P;
-        veh0.assign(P, make_int2(0, 0)); veh1.assign(P, make_int2(0, 0)); act0.assign(nD, 0); act1.assign(nD, 0); extra.assign(nD, 0);
-        V.finCap = 1 << 16;
-        finSlots.assign(V.finCap, make_int2(0, 0));
+        P = L.P;
         slotCap = 1 << 17;
-        pos.assign(slotCap, -1); waitNext.assign(slotCap, -1); slotInfo.assign(slotCap, make_int4(0, 0, 0, 0)); slotCust.assign(slotCap, NAN);
-        blk.assign(slotCap, -1); delStep.assign(slotCap, INT_MIN);
-        tmpl.assign(slotCap, DTmpl{});
-        spawn.assign(1 << 14, SpawnRec{});
-        // lane change
-        segBeg.assign(nL + 1, 0); laneIdx.resize(nL); laneRoadN.resize(nL); laneWidth.resize(nL);
-        for (int l = 0; l < nL; ++l) {
-            segBeg[l] = (int) segStart.size();
-            for (double x : segStartPerLane[l]) segStart.push_back(x);
-            laneIdx[l] = net.laneIdx[l]; laneRoadN[l] = net.roadNumLanes(net.laneRoad[l]); laneWidth[l] = net.laneWidth[l];
-        }
-        segBeg[nL] = (int) segStart.size();
-        posDrv.resize(P);
-        for (int d = 0; d < nD; ++d) for (int p = off[d]; p < off[d + 1]; ++p) posDrv[p] = d;
-        segIdx.assign(P, 0); cand.assign(LC_MAX_CAND, 0); involved.assign(LC_MAX_CAND, 0); shadowLog.assign(LC_MAX_CAND, make_int2(0, 0));
-        prio.assign(LC_MAX_CAND, 0); lcSlot.assign(slotCap, LcSlot{}); spare.assign(256, 0);
+        kin.resize(P); nkin.resize(P); gap.resize(P); leader.resize(P); ids.resize(P); nav.resize(P); nbuf.resize(P); cust.resize(P);
+        count.resize(nD); entCnt.resize(nD); ent.resize((size_t) nD * ENT_CAP);
+        waitHead.resize(std::max(nL, 1)); waitTail.resize(std::max(nL, 1)); inserted.resize(std::max(nL, 1));
+        notify.resize(std::max(2 * net.nCross(), 1));
+        curPhase.resize(net.nInter()); remain.resize(net.nInter()); rlAvail.resize(std::max(net.nRoadLinks(), 1));
+        mkin.resize(V.moverCap); mids.resize(V.moverCap); mnav.resize(V.moverCap);
+        tail.resize(nD); foeMask.resize((size_t) std::max(nK, 1) * V.maskWords);
+        veh0.resize(P); veh1.resize(P); act0.resize(nD); act1.resize(nD); extra.resize(nD);
+        finSlots.resize(V.finCap);
+        pos.resize(slotCap); waitNext.resize(slotCap); slotInfo.resize(slotCap); slotCust.resize(slotCap); blk.resize(slotCap); delStep.resize(slotCap);
+        tmpl.resize(slotCap);
+        spawn.resize(1 << 14);
+        segIdx.resize(P); cand.resize(LC_MAX_CAND); involved.resize(LC_MAX_CAND); shadowLog.resize(LC_MAX_CAND); prio.resize(LC_MAX_CAND);
+        lcSlot.resize(slotCap); spare.resize(256); scratch.resize((size_t) 4 * LC_MAX_CAND);
         // pointers
-        V.drvLength = drvLength.p(); V.drvMaxSpeed = drvMaxSpeed.p(); V.off = off.p(); V.laneOutBeg = laneOutBeg.p(); V.laneOutLinks = laneOutLinks.p();
-        V.llStartLane = llStartLane.p(); V.llEndLane = llEndLane.p(); V.llRoadLink = llRoadLink.p(); V.linkInfo = linkInfo.p();
-        V.llCrossBeg = llCrossBeg.p(); V.lcIdx = lcIdx.p(); V.lcDist = lcDist.p(); V.csLink = csLink.p(); V.lcPeer = lcPeer.p();
-        V.interPhaseBeg = interPhaseBeg.p(); V.interRLBeg = interRLBeg.p(); V.phaseAvailBeg = phaseAvailBeg.p(); V.rlInter = rlInter.p();
-        V.phaseTime = phaseTime.p(); V.phaseAvail = phaseAvail.p(); V.interVirtual = interVirtual.p(); V.tmpl = tmpl.p();
+        V.drvLength = L.drvLength.data(); V.drvMaxSpeed = L.drvMaxSpeed.data(); V.off = L.off.data();
+        V.laneOutBeg = L.laneOutBeg.data(); V.laneOutLinks = L.laneOutLinks.data();
+        V.llStartLane = L.llStartLane.data(); V.llEndLane = L.llEndLane.data(); V.llRoadLink = L.llRoadLink.data(); V.linkInfo = L.linkInfo.data();
+        V.llCrossBeg = L.llCrossBeg.data(); V.lcIdx = L.lcIdx.data(); V.lcDist = L.lcDist.data(); V.lcPeer = L.lcPeer.data(); V.csLink = L.csLink.data();
+        V.interPhaseBeg = L.interPhaseBeg.data(); V.interRLBeg = L.interRLBeg.data(); V.phaseAvailBeg = L.phaseAvailBeg.data();
+        V.rlInter = L.rlInter.data(); V.phaseTime = L.phaseTime.data(); V.phaseAvail = L.phaseAvail.data(); V.interVirtual = L.interVirtual.data();
+        V.tmpl = tmpl.p();
         V.kin = kin.p(); V.nkin = nkin.p(); V.gap = gap.p(); V.leader = leader.p(); V.ids = ids.p(); V.nav = nav.p(); V.nbuf = nbuf.p();
         V.count = count.p(); V.pos = pos.p(); V.waitHead = waitHead.p(); V.waitTail = waitTail.p(); V.waitNext = waitNext.p();
         V.slotInfo = slotInfo.p(); V.inserted = inserted.p(); V.notify = notify.p(); V.tail = tail.p(); V.foeMask = foeMask.p();
@@ -147,23 +90,23 @@ struct HostSim {   // DeviceSim's arrays (device_sim.cu constructor), on the hos
         V.cust = cust.p(); V.slotCust = slotCust.p(); V.blk = blk.p(); V.delStep = delStep.p(); V.ctrl = &ctrl;
         V.lcOn = laneChange ? 1 : 0;
         LcView &C = V.lc;
-        C.slot = lcSlot.p(); C.segIdx = segIdx.p(); C.posDrv = posDrv.p(); C.segBeg = segBeg.p(); C.segStart = segStart.p();
-        laneRoadT.assign(net.laneRoad.begin(), net.laneRoad.end()); C.laneRoad = laneRoadT.p();
-        C.laneIdx = laneIdx.p(); C.laneRoadN = laneRoadN.p(); C.laneWidth = laneWidth.p(); C.cand = cand.p(); C.involved = involved.p();
-        C.spare = spare.p(); C.nSpare = 0; C.shadowLog = shadowLog.p(); C.ctrl = &lcCtrl;
-        scratch.assign((size_t) 4 * LC_MAX_CAND, 0);
+        C.slot = lcSlot.p(); C.segIdx = segIdx.p(); C.posDrv = L.posDrv.data(); C.segBeg = L.segBeg.data(); C.segStart = L.segStart.data();
+        C.laneRoad = L.laneRoad.data(); C.laneIdx = L.laneIdx.data(); C.laneRoadN = L.laneRoadN.data(); C.laneWidth = L.laneWidth.data();
+        C.cand = cand.p(); C.involved = involved.p(); C.spare = spare.p(); C.nSpare = 0; C.shadowLog = shadowLog.p(); C.ctrl = &lcCtrl;
         C.scratchA = scratch.p(); C.scratchB = scratch.p() + LC_MAX_CAND; C.scratchC = scratch.p() + 2 * LC_MAX_CAND; C.scratchD = scratch.p() + 3 * LC_MAX_CAND;
+        reset();
+    }
+    void reset() {   // DeviceSim::reset with memset for cudaMemset
+        for (const Fill &f : resetFills(V, (size_t) P, (size_t) slotCap)) memset(f.p, f.byte, f.bytes);
+        std::copy(L.remain0.begin(), L.remain0.end(), remain.begin());
     }
     void setPlans(const Routing &R) {
-        planBeg.assign(R.planBeg().begin(), R.planBeg().end()); planData.assign(R.planData().begin(), R.planData().end());
-        planRoute.assign(R.planRouteTable().begin(), R.planRouteTable().end()); planRoadPos.assign(R.planRoadPosTable().begin(), R.planRoadPosTable().end());
-        lpRoad.assign(R.lanePlanRoadTable().begin(), R.lanePlanRoadTable().end()); lpBeg.assign(R.lanePlanBegTable().begin(), R.lanePlanBegTable().end());
-        lpId.assign(R.lanePlanIdTable().begin(), R.lanePlanIdTable().end());
-        routeLast.assign(std::max(R.numRoutes(), 1), -1);
-        for (int r = 0; r < R.numRoutes(); ++r) if (R.route(r).valid) routeLast[r] = R.route(r).roads.back();
-        V.lc.routeLastRoad = routeLast.p();
-        V.planBeg = planBeg.p(); V.planData = planData.p();
-        V.lc.planRoute = planRoute.p(); V.lc.planRoadPos = planRoadPos.p(); V.lc.lanePlanRoad = lpRoad.p(); V.lc.lanePlanBeg = lpBeg.p(); V.lc.lanePlanId = lpId.p();
+        plans = planTables(R);
+        lanePlans = lanePlanTables(R);
+        V.planBeg = plans.planBeg.data(); V.planData = plans.planData.data();
+        LcView &C = V.lc;
+        C.planRoute = lanePlans.planRoute.data(); C.planRoadPos = lanePlans.planRoadPos.data(); C.lanePlanRoad = lanePlans.lanePlanRoad.data();
+        C.lanePlanBeg = lanePlans.lanePlanBeg.data(); C.lanePlanId = lanePlans.lanePlanId.data(); C.routeLastRoad = lanePlans.routeLastRoad.data();
     }
     template <class F> void run(int nBlocks, F f) {
         gridDim.x = (unsigned) nBlocks;

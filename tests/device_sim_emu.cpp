@@ -13,7 +13,6 @@
 // a loop-back group.  Not emulated (throw): NCCL sharding, device-resident observations / actions, timing.
 #include "device_hostsim.h"
 #include "device_image.cuh"
-#include "partition.h"
 
 #include <stdexcept>
 
@@ -26,7 +25,6 @@ struct DeviceSim::Impl {
     DeviceSimOptions opt;
     std::vector<int> hPhase;
     bool phaseDirty = false;
-    std::vector<int> offHost;
 };
 
 // ---- sharding over "peer memory": the ranks of a loop-back group (host_engine.cpp cfb_shard_group_*) live in one process, a
@@ -42,13 +40,14 @@ struct EmuArena {   // what DeviceSim::shardArena() hands out here: where a peer
 struct ShardEmu {
     int rank = 0, world = 1;
     std::vector<std::vector<int>> bsize;
-    cfbtest::Buf<unsigned char> owned;
-    cfbtest::Buf<int> boundOut, boundIn, ing, flags, ints;
+    std::vector<unsigned char> owned;   // per drivable: 1 = this rank's (debugDump)
+    ShardLists lists;
+    cfbtest::Buf<int> flags;
+    std::vector<int> ints;
     cfbtest::Buf<int2> blkUpd, blkIn;
     cfbtest::Buf<MoverMsg> moverIn;
     cfbtest::Buf<TailMsg> tailIn;
     cfbtest::Buf<ShardPeer> peers;
-    std::vector<unsigned char> ownedHost;
     EmuArena arena{};
     ShardP2P S{};
     bool connected = false;
@@ -57,15 +56,6 @@ static std::map<const DeviceSim *, ShardEmu> g_shardEmu;
 
 
 static void notEmulated(const char *what) { throw std::runtime_error(std::string("device_sim_emu: ") + what + " is not emulated"); }
-
-static DTmpl toDevice(const VehicleTemplate &t, double interval) {   // same as device_sim.cu
-    DTmpl d{};
-    d.len = t.len; d.maxPosAcc = t.maxPosAcc; d.maxNegAcc = t.maxNegAcc; d.usualPosAcc = t.usualPosAcc; d.usualNegAcc = t.usualNegAcc;
-    d.minGap = t.minGap; d.maxSpeed = t.maxSpeed; d.headwayTime = t.headwayTime; d.yieldDistance = t.yieldDistance; d.turnSpeed = t.turnSpeed;
-    d.approachDist = t.maxSpeed * t.maxSpeed / t.usualNegAcc / 2 + t.maxSpeed * interval * 2;
-    d.speed0 = t.speed;
-    return d;
-}
 
 DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &templates, const Routing &routing, const DeviceSimOptions &opt)
     : impl_(new Impl()) {
@@ -77,24 +67,10 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
     }
     Impl &I = *impl_;
     I.opt = opt;
-    // segment boundaries (DeviceSim::enableLaneChange): computed always, used only with laneChange
-    std::vector<std::vector<double>> seg(net.nLanes());
-    for (int r = 0; r < net.nRoads(); ++r) {
-        double len = 0.0;
-        const auto &pts = net.roadPoints[r];
-        for (size_t i = 0; i + 1 < pts.size(); ++i) {
-            const double dx = pts[i + 1].x - pts[i].x, dy = pts[i + 1].y - pts[i].y;
-            len += sqrt(dx * dx + dy * dy);
-        }
-        const size_t numSegs = std::max((size_t) ceil(len / ((5.0 + 2.0) * 10)), (size_t) 1);
-        for (int l = net.roadLaneBeg[r]; l < net.roadLaneBeg[r + 1]; ++l)
-            for (size_t i = 0; i < numSegs; ++i) seg[l].push_back(i * net.laneLength[l] / numSegs);
-    }
-    I.H.init(net, opt.interval, opt.rlTrafficLight, false, seg);
-    I.offHost.assign(I.H.off.begin(), I.H.off.end());
-    I.hPhase.assign(net.nInter(), 0);
+    I.H.init(net, opt.interval, opt.rlTrafficLight, false);
     uploadTemplates(templates);
     uploadPlans(routing);
+    reset();
 }
 DeviceSim::~DeviceSim() {
     g_shardEmu.erase(this);   // (a later engine at the same address must not inherit this one's mailboxes and flags)
@@ -105,16 +81,7 @@ void DeviceSim::uploadTemplates(const std::vector<VehicleTemplate> &templates) {
     HostSim &H = impl_->H;
     for (size_t k = 0; k < templates.size(); ++k) H.tmpl[k] = toDevice(templates[k], impl_->opt.interval);
 }
-void DeviceSim::uploadPlans(const Routing &routing) {
-    HostSim &H = impl_->H;
-    H.planBeg.assign(routing.planBeg().begin(), routing.planBeg().end());
-    H.planData.assign(routing.planData().begin(), routing.planData().end());
-    if (H.planBeg.empty()) H.planBeg.push_back(0);
-    if (H.planData.empty()) H.planData.push_back(PLAN_END);
-    H.V.planBeg = H.planBeg.p();
-    H.V.planData = H.planData.p();
-    if (H.V.lcOn) uploadLanePlans(routing);
-}
+void DeviceSim::uploadPlans(const Routing &routing) { impl_->H.setPlans(routing); }
 void DeviceSim::ensureSlotCapacity(int slots) {
     if (getenv("CFB_EMU_HOST_ONLY")) return;
     if (slots > impl_->H.slotCap) throw std::runtime_error("device_sim_emu: slot capacity of the emulated device exceeded");
@@ -217,7 +184,7 @@ void DeviceSim::laneWaitingVehicleCount(int32_t *out) {
     HostSim &H = impl_->H;
     for (int l = 0; l < H.V.nLanes; ++l) {
         int c = 0;
-        for (int k = 0; k < H.count[l]; ++k) c += H.kin[H.off[l] + k].y < 0.1;
+        for (int k = 0; k < H.count[l]; ++k) c += H.kin[H.L.off[l] + k].y < 0.1;
         out[l] = c;
     }
 }
@@ -226,7 +193,7 @@ int DeviceSim::runningVehicles(std::vector<SpeedRec> &out) {
     out.clear();
     for (int d = 0; d < H.V.nDrv; ++d)
         for (int k = 0; k < H.count[d]; ++k) {
-            const int p = H.off[d] + k;
+            const int p = H.L.off[d] + k;
             out.push_back(SpeedRec{H.ids[p].x, d, H.kin[p].y, H.kin[p].x});
         }
     return (int) out.size();
@@ -251,74 +218,22 @@ int DeviceSim::device() const { return -1; }
 unsigned long long DeviceSim::vehicleSteps() { return impl_->H.ctrl.vehicleSteps; }
 
 void DeviceSim::reset() {
-    HostSim &H = impl_->H;
-    std::fill(H.count.begin(), H.count.end(), 0); std::fill(H.entCnt.begin(), H.entCnt.end(), 0);
-    std::fill(H.waitHead.begin(), H.waitHead.end(), -1); std::fill(H.waitTail.begin(), H.waitTail.end(), -1);
-    std::fill(H.inserted.begin(), H.inserted.end(), 0);
-    std::fill(H.pos.begin(), H.pos.end(), -1); std::fill(H.waitNext.begin(), H.waitNext.end(), -1);
-    std::fill(H.cust.begin(), H.cust.end(), NAN); std::fill(H.slotCust.begin(), H.slotCust.end(), NAN);
-    std::fill(H.blk.begin(), H.blk.end(), -1); std::fill(H.delStep.begin(), H.delStep.end(), INT_MIN);
-    for (auto &n : H.notify) n = Notify{0.0, 0, 0};
-    Tail empty{}; empty.pos = -1; empty.prev = -1;
-    std::fill(H.tail.begin(), H.tail.end(), empty);
-    std::fill(H.foeMask.begin(), H.foeMask.end(), 0u);
-    std::fill(H.curPhase.begin(), H.curPhase.end(), 0);
-    std::fill(impl_->hPhase.begin(), impl_->hPhase.end(), 0);
+    impl_->H.reset();
+    impl_->hPhase.assign(impl_->H.V.nInter, 0);
     impl_->phaseDirty = false;
-    for (int i = 0; i < H.V.nInter; ++i) H.remain[i] = H.interVirtual[i] ? 0.0 : H.phaseTime[H.interPhaseBeg[i]];
-    std::fill(H.rlAvail.begin(), H.rlAvail.end(), 0);
-    H.ctrl = Ctrl{};
     steps_ = 0;
 }
 
 void DeviceSim::debugDump(std::vector<DebugRec> &out) {
-    HostSim &H = impl_->H;
-    const int lastStep = H.ctrl.step - 1;
-    out.clear();
-    const std::vector<unsigned char> *ownedHost = nullptr;   // one rank of a loop-back group: its own drivables only (the rest holds ghost data)
-    {
-        auto it = g_shardEmu.find(this);
-        if (it != g_shardEmu.end() && !it->second.ownedHost.empty()) ownedHost = &it->second.ownedHost;
-    }
-    for (int d = 0; d < H.V.nDrv; ++d)
-        for (int k = 0; k < H.count[d]; ++k) {
-            if (ownedHost && !(*ownedHost)[d]) break;
-            const int p = H.off[d] + k;
-            DebugRec r{};
-            r.slot = H.ids[p].x; r.drivable = d;
-            r.leaderSlot = H.leader[p] >= 0 ? H.ids[H.leader[p]].x : -1;
-            r.blockerSlot = H.nav[p].z;
-            if (r.blockerSlot >= 0 && H.delStep[r.blockerSlot] == lastStep) r.blockerSlot = -1;
-            r.priority = H.ids[p].z; r.enterLaneLinkTime = H.nav[p].w; r.listIndex = k;
-            r.dis = H.kin[p].x; r.speed = H.kin[p].y; r.gap = H.leader[p] >= 0 ? H.gap[p] : 0.0;
-            out.push_back(r);
-        }
+    auto it = g_shardEmu.find(this);   // one rank of a loop-back group: its own drivables only (the rest holds ghost data)
+    debugRecords(impl_->H.V, it != g_shardEmu.end() && !it->second.owned.empty() ? it->second.owned.data() : nullptr, out);
 }
-void DeviceSim::debugDumpLc(std::vector<LcDebugRec> &out) {
-    HostSim &H = impl_->H;
-    const int lastStep = H.ctrl.step - 1;
-    out.clear();
-    for (int d = 0; d < H.V.nDrv; ++d)
-        for (int k = 0; k < H.count[d]; ++k) {
-            const int p = H.off[d] + k;
-            const LcSlot &L = H.lcSlot[H.ids[p].x];
-            LcDebugRec r{};
-            r.slot = H.ids[p].x; r.priority = H.ids[p].z; r.partnerType = L.type; r.partnerSlot = L.partner; r.drivable = d;
-            r.leaderSlot = H.leader[p] >= 0 ? H.ids[H.leader[p]].x : -1;
-            r.blockerSlot = H.nav[p].z;
-            if (r.blockerSlot >= 0 && H.delStep[r.blockerSlot] == lastStep) r.blockerSlot = -1;
-            r.flags = L.changing | (L.finished << 1);
-            r.lastDir = L.lastDir;
-            r.dis = H.kin[p].x; r.speed = H.kin[p].y; r.gap = H.leader[p] >= 0 ? L.gap : 0.0;
-            r.offset = L.offset; r.waiting = L.waiting; r.lastChange = L.lastChange;
-            out.push_back(r);
-        }
-}
+void DeviceSim::debugDumpLc(std::vector<LcDebugRec> &out) { lcDebugRecords(impl_->H.V, out); }
 bool DeviceSim::vehicleState(int slot, VehState &out) {
     HostSim &H = impl_->H;
     if (slot < 0 || slot >= H.slotCap || H.pos[slot] < 0) return false;
     const int p = H.pos[slot];
-    out.pos = p; out.drivable = H.posDrv[p]; out.planIdx = H.nav[p].x; out.nextDrv = H.ids[p].w; out.dis = H.kin[p].x; out.speed = H.kin[p].y;
+    out.pos = p; out.drivable = H.L.posDrv[p]; out.planIdx = H.nav[p].x; out.nextDrv = H.ids[p].w; out.dis = H.kin[p].x; out.speed = H.kin[p].y;
     return true;
 }
 int DeviceSim::leaderSlotOf(int slot) {
@@ -332,7 +247,7 @@ void DeviceSim::laneVehicleSlots(std::vector<int32_t> &slots, std::vector<int32_
     laneBeg.assign(H.V.nLanes + 1, 0);
     slots.clear();
     for (int l = 0; l < H.V.nLanes; ++l) {
-        for (int k = 0; k < H.count[l]; ++k) slots.push_back(H.ids[H.off[l] + k].x);
+        for (int k = 0; k < H.count[l]; ++k) slots.push_back(H.ids[H.L.off[l] + k].x);
         laneBeg[l + 1] = (int) slots.size();
     }
 }
@@ -352,31 +267,11 @@ void DeviceSim::configureShard(int rank, int world, const std::vector<unsigned c
                                const std::vector<std::vector<int>> &ownPerPeer, const std::vector<std::vector<int>> &boundarySize,
                                const std::vector<unsigned char> &ownedRoadLinks) {
     ShardEmu &E = g_shardEmu[this];
-    HostSim &H = impl_->H;
-    View &V = H.V;
-    E.rank = rank; E.world = world; E.bsize = boundarySize; E.ownedHost = owned;
-    std::vector<unsigned char> own3 = owned;
-    for (int q = 0; q < world; ++q) for (int l : feedPerPeer[q]) own3[l] = 2;
-    E.owned.assign(own3.begin(), own3.end());
-    V.owned = E.owned.p();
-    std::vector<int> lanes, links, rls;
-    for (int l = 0; l < V.nLanes; ++l) if (own3[l]) lanes.push_back(l);
-    for (int k = 0; k < V.nLinks; ++k) if (owned[V.nLanes + k]) links.push_back(k);
-    for (int r = 0; r < (int) ownedRoadLinks.size(); ++r) if (ownedRoadLinks[r]) rls.push_back(r);
-    V.nIngLanes = (int) lanes.size(); V.nIngLinks = (int) links.size(); V.nIngRL = (int) rls.size();
-    E.ing.clear();
-    E.ing.insert(E.ing.end(), lanes.begin(), lanes.end()); E.ing.insert(E.ing.end(), links.begin(), links.end()); E.ing.insert(E.ing.end(), rls.begin(), rls.end());
-    E.ing.push_back(0);
-    V.ingLanes = E.ing.p(); V.ingLinks = E.ing.p() + lanes.size(); V.ingRL = E.ing.p() + lanes.size() + links.size();
-    E.boundOut.clear(); E.boundIn.clear();
-    for (int q = 0; q < world; ++q) {
-        E.boundOut.insert(E.boundOut.end(), feedPerPeer[q].begin(), feedPerPeer[q].end());
-        E.boundIn.insert(E.boundIn.end(), ownPerPeer[q].begin(), ownPerPeer[q].end());
-    }
-    V.nBoundOut = (int) E.boundOut.size(); V.nBoundIn = (int) E.boundIn.size();
-    if (E.boundOut.empty()) E.boundOut.push_back(0);
-    if (E.boundIn.empty()) E.boundIn.push_back(0);
-    V.boundOut = E.boundOut.p(); V.boundIn = E.boundIn.p();
+    View &V = impl_->H.V;
+    E.rank = rank; E.world = world; E.bsize = boundarySize; E.owned = owned;
+    E.lists = shardLists(V.nLanes, V.nLinks, owned, feedPerPeer, ownPerPeer, ownedRoadLinks);
+    V.owned = E.lists.owned.data();
+    E.lists.point(V, E.lists.ing.data(), E.lists.boundOut.data(), E.lists.boundIn.data());
     V.blkUpdCap = BLK_IN_CAP;
     E.blkUpd.assign(1 + V.blkUpdCap, make_int2(0, 0));
     V.blkUpd = E.blkUpd.p();
@@ -403,16 +298,11 @@ void DeviceSim::shardConnect(const std::vector<void *> &peerBase) {
         P.flags = A.flags; P.delStep = A.delStep; P.blkIn = A.blkIn + (size_t) me * (1 + BLK_IN_CAP);
         P.moverIn = A.moverIn; P.tailIn = A.tailIn; P.nIn = A.nIn; P.nOut = A.nOut;
     }
-    const SeamTables T = seamTables(E.bsize, me);
-    E.ints.clear();
-    const size_t oN = 0, oOP = oN + T.nbr.size(), oOD = oOP + T.outPeer.size(), oIP = oOD + T.outDst.size(), oID = oIP + T.inPeer.size(), oT = oID + T.inDst.size();
-    for (const std::vector<int> *v : {&T.nbr, &T.outPeer, &T.outDst, &T.inPeer, &T.inDst}) E.ints.insert(E.ints.end(), v->begin(), v->end());
-    E.ints.push_back(0); E.ints.push_back(0);
+    const SeamIndex X = seamIndex(seamTables(E.bsize, me));
+    E.ints = X.ints;
     ShardP2P &S = E.S;
     S.peers = E.peers.p(); S.me = me; S.world = W;
-    S.nbr = E.ints.p() + oN; S.nNbr = (int) T.nbr.size();
-    S.outPeer = E.ints.p() + oOP; S.outDst = E.ints.p() + oOD; S.inPeer = E.ints.p() + oIP; S.inDst = E.ints.p() + oID;
-    S.ticket = E.ints.p() + oT;
+    X.point(S, E.ints.data());
     S.flags = E.flags.p(); S.blkIn = E.blkIn.p(); S.moverIn = E.moverIn.p(); S.tailIn = E.tailIn.p();
     E.connected = true;
 }
@@ -460,52 +350,42 @@ DeviceSim::Snapshot *DeviceSim::snapshot() {
     HostSim &H = I.H;
     if (I.phaseDirty) { for (int i = 0; i < H.V.nInter; ++i) H.curPhase[i] = I.hPhase[i]; I.phaseDirty = false; }
     const auto regs = snapshotRegions(H.V, (size_t) H.P, (size_t) H.slotCap);
-    std::vector<long long> hdr = {IMAGE_MAGIC, steps_, (long long) H.slotCap, (long long) regs.size()};
-    size_t total = 0;
-    for (auto &r : regs) { hdr.push_back((long long) r.second); total += imagePad(r.second); }
+    const ImageHeader h = imageHeader(steps_, H.slotCap, regs);
     Snapshot *s = new Snapshot();
-    s->bytes.assign(hdr.size() * sizeof(long long) + total, 0);
-    memcpy(s->bytes.data(), hdr.data(), hdr.size() * sizeof(long long));
-    size_t off = hdr.size() * sizeof(long long);
+    s->bytes.assign(h.bytes() + h.payload(), 0);
+    writeImageHeader(h, s->bytes.data());
+    size_t off = h.bytes();
     for (auto &r : regs) { if (r.second) memcpy(s->bytes.data() + off, r.first, r.second); off += imagePad(r.second); }
     return s;
 }
 void DeviceSim::restore(const Snapshot *s) {
     Impl &I = *impl_;
     HostSim &H = I.H;
-    const long long *h = reinterpret_cast<const long long *>(s->bytes.data());
-    const int slotCap = (int) h[2];
-    ensureSlotCapacity(slotCap);
+    const ImageHeader h = readImageHeader(s->bytes.data(), s->bytes.size());
+    ensureSlotCapacity(h.slotCap);
     const auto regs = snapshotRegions(H.V, (size_t) H.P, (size_t) H.slotCap);
-    if ((size_t) h[3] != regs.size()) throw std::runtime_error("cityflow_b200: archive does not match this engine");
-    std::fill(H.pos.begin(), H.pos.end(), -1); std::fill(H.waitNext.begin(), H.waitNext.end(), -1);
-    std::fill(H.slotCust.begin(), H.slotCust.end(), NAN); std::fill(H.blk.begin(), H.blk.end(), -1);
-    std::fill(H.delStep.begin(), H.delStep.end(), INT_MIN);
-    size_t off = (4 + regs.size()) * sizeof(long long);
+    checkImageFits(h, regs, H.V);
+    for (const Fill &f : slotFills(H.V, (size_t) H.slotCap)) memset(f.p, f.byte, f.bytes);
+    size_t off = h.bytes();
     for (size_t k = 0; k < regs.size(); ++k) {
-        const size_t bytes = (size_t) h[4 + k];
-        if (bytes > regs[k].second) throw std::runtime_error("cityflow_b200: archive does not match this engine (region size)");
-        if (k + imageSlotRegions(H.V) < regs.size() && bytes != regs[k].second) throw std::runtime_error("cityflow_b200: archive was taken on a different road network");
-        if (bytes) memcpy(regs[k].first, s->bytes.data() + off, bytes);
-        off += imagePad(bytes);
+        if (h.regions[k]) memcpy(regs[k].first, s->bytes.data() + off, h.regions[k]);
+        off += imagePad(h.regions[k]);
     }
     for (int i = 0; i < H.V.nInter; ++i) I.hPhase[i] = H.curPhase[i];
     I.phaseDirty = false;
-    for (auto &n : H.notify) n = Notify{0.0, 0, 0};
-    std::fill(H.foeMask.begin(), H.foeMask.end(), 0u);
-    steps_ = h[1];
+    for (const Fill &f : scratchFills(H.V)) memset(f.p, f.byte, f.bytes);
+    steps_ = h.steps;
 }
 void DeviceSim::freeSnapshot(Snapshot *s) { delete s; }
 void DeviceSim::snapshotToHost(const Snapshot *s, std::vector<unsigned char> &out) { out = s->bytes; }
 DeviceSim::Snapshot *DeviceSim::snapshotFromHost(const unsigned char *data, size_t n) {
-    if (n < 4 * sizeof(long long) || reinterpret_cast<const long long *>(data)[0] != IMAGE_MAGIC)
-        throw std::runtime_error("cityflow_b200: not an archive of this engine");
+    readImageHeader(data, n);
     Snapshot *s = new Snapshot();
     s->bytes.assign(data, data + n);
     return s;
 }
 static ImageGeometry imageGeometry(DeviceSim::Impl &I) {
-    return ImageGeometry{I.offHost.data(), I.H.V.nDrv, I.H.V.nLanes, I.H.V.nInter, (size_t) I.H.P};
+    return ImageGeometry{I.H.L.off.data(), I.H.V.nDrv, I.H.V.nLanes, I.H.V.nInter, (size_t) I.H.P};
 }
 void DeviceSim::decodeSnapshot(const Snapshot *s, StateImage &out) {
     std::vector<unsigned char> blob;

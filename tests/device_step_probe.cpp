@@ -3,8 +3,9 @@
 // The bodies of all five step kernels (csrc/device_phases_a.cuh: k_ingest, k_notify; device_control.cuh:
 // k_control; device_phases_b.cuh: k_move, k_leader) and, with laneChange, the lane-change kernels
 // (csrc/device_lc.cuh) run on an emulated warp (tests/device_emu.h: 32 lock-stepped fibers) over
-// persistent lane-bucket arrays laid out like DeviceSim's.  The emulated engine gets the same spawn events as
-// the restatement (oracle/cityflow_oracle.cpp) and evolves ON ITS OWN; after every step its full state --
+// persistent lane-bucket arrays laid out by DeviceSim's own layout code (csrc/device_layout.cuh).  The emulated
+// engine gets the same spawn events as the restatement (oracle/cityflow_oracle.cpp) and evolves ON ITS OWN; after
+// every step its full state --
 // list order, distance, speed, leader, gap, blocker, enterLaneLinkTime of every vehicle, vehicle counts,
 // finished vehicles, and with laneChange every shadow, partner link, offset, waiting time -- must equal the
 // restatement's.  That is the GPU parity test (tests/test_gpu_parity.py) minus the GPU: it checks the
@@ -66,13 +67,8 @@ void deviceStep(Oracle &o) {
         r.slot = s; r.lane = v->firstLaneForProbe; r.tmpl = s; r.priority = v->priority;
         r.plan = R.lanePlan(route, 0, o.net.laneIdx[r.lane]);
         recs.push_back(r);
-        DTmpl t{};   // toDevice() of device_sim.cu
-        t.len = v->t.len; t.maxPosAcc = v->t.maxPosAcc; t.maxNegAcc = v->t.maxNegAcc; t.usualPosAcc = v->t.usualPosAcc;
-        t.usualNegAcc = v->t.usualNegAcc; t.minGap = v->t.minGap; t.maxSpeed = v->t.maxSpeed; t.headwayTime = v->t.headwayTime;
-        t.yieldDistance = v->t.yieldDistance; t.turnSpeed = v->t.turnSpeed;
-        t.approachDist = v->t.maxSpeed * v->t.maxSpeed / v->t.usualNegAcc / 2 + v->t.maxSpeed * o.interval * 2;
-        t.speed0 = v->initialSpeedForProbe;
-        H.tmpl[s] = t;
+        H.tmpl[s] = toDevice(v->t, o.interval);
+        H.tmpl[s].speed0 = v->initialSpeedForProbe;
     }
     std::stable_sort(recs.begin(), recs.end(), [](const SpawnRec &a, const SpawnRec &b) { return a.lane < b.lane; });
     H.setPlans(R);   // (routes are interned lazily: tables may have grown)
@@ -95,24 +91,24 @@ void deviceStep(Oracle &o) {
                 const int s = slotOf.at(kv.second), p = H.pos[s];
                 if (p < 0) continue;
                 const LcSlot &L = H.lcSlot[s];
-                const int dd = H.posDrv[p];
+                const int dd = H.L.posDrv[p];
                 const int rp = lcRoadPos(V, V.lc, L.plan, H.nav[p].x);
-                printf("  signal step %zu: drivable %d laneIdx %d/%d dis %.4f own gap %.6f len %.2f seg %d plan %d planIdx %d roadPos %d next %d -> target %d epoch %d\n", o.step, dd, H.laneIdx[dd],
-                       H.laneRoadN[dd], H.kin[p].x, L.gap, H.tmpl[H.ids[p].y].len, H.segIdx[p], L.plan, H.nav[p].x, rp, H.ids[p].w, L.sendTarget, L.sendEpoch);
+                printf("  signal step %zu: drivable %d laneIdx %d/%d dis %.4f own gap %.6f len %.2f seg %d plan %d planIdx %d roadPos %d next %d -> target %d epoch %d\n", o.step, dd, H.L.laneIdx[dd],
+                       H.L.laneRoadN[dd], H.kin[p].x, L.gap, H.tmpl[H.ids[p].y].len, H.segIdx[p], L.plan, H.nav[p].x, rp, H.ids[p].w, L.sendTarget, L.sendEpoch);
                 {
                     Veh *v = kv.second;
                     printf("    restatement: iCur %d route size %zu onLastRoad %d; routerNextOf(outer) %d; plan's route %d roads:", v->iCur, v->route.size(), (int) o.onLastRoad(*v),
-                           dd + 1 < V.nLanes ? o.routerNextOf(*v, dd + 1) : -9, H.planRoute[L.plan]);
+                           dd + 1 < V.nLanes ? o.routerNextOf(*v, dd + 1) : -9, H.lanePlans.planRoute[L.plan]);
                     for (int r2 : v->route) printf(" %d", r2);
                     printf(" | lane road %d; lanePlan ids for roadPos %d:", o.net.laneRoad[dd], rp);
-                    for (int k2 = 0; k2 < H.laneRoadN[dd]; ++k2) { const int np = lcLanePlan(V.lc, L.plan, rp, dd - H.laneIdx[dd] + k2); printf(" %d(next %d)", np, H.planData[H.planBeg[np] + 1]); }
+                    for (int k2 = 0; k2 < H.L.laneRoadN[dd]; ++k2) { const int np = lcLanePlan(V.lc, L.plan, rp, dd - H.L.laneIdx[dd] + k2); printf(" %d(next %d)", np, H.plans.planData[H.plans.planBeg[np] + 1]); }
                     printf("\n");
                 }
                 for (int adj : {dd + 1, dd - 1}) {
                     if (adj < 0 || adj >= V.nLanes || o.net.laneRoad[adj] != o.net.laneRoad[dd]) continue;
                     const int lp = lcVehicleAfter(V, V.lc, adj, H.kin[p].x, H.segIdx[p]);
                     printf("    lane %d: continues %d, vehicle ahead pos %d est %.4f (count %d)\n", adj, (int) lcLaneContinues(V, V.lc, L.plan, rp, adj, H.ids[p].w == -1), lp,
-                           lp < 0 ? H.drvLength[adj] - H.kin[p].x : H.kin[lp].x - H.kin[p].x - H.tmpl[H.ids[lp].y].len, H.count[adj]);
+                           lp < 0 ? H.L.drvLength[adj] - H.kin[p].x : H.kin[lp].x - H.kin[p].x - H.tmpl[H.ids[lp].y].len, H.count[adj]);
                 }
             }
         }
@@ -162,10 +158,10 @@ void deviceStep(Oracle &o) {
             const int want = atoi(tp);
             for (int k = 0; k < ns; ++k) if (H.prio[k] == want) {
                 const int sh = H.shadowLog[k].y, p = H.pos[sh];
-                printf("  mid-step: shadow slot %d at pos %d (drivable %d, count %d) next %d planIdx %d leader %d V.gap %.6f own %.6f; nAct %d; parent tgtLeader %d\n", sh, p, H.posDrv[p],
-                       H.count[H.posDrv[p]], H.ids[p].w, H.nav[p].x, H.leader[p], H.gap[p], H.lcSlot[sh].gap, H.ctrl.nAct[V.par], H.lcSlot[H.shadowLog[k].x].tgtLeader);
+                printf("  mid-step: shadow slot %d at pos %d (drivable %d, count %d) next %d planIdx %d leader %d V.gap %.6f own %.6f; nAct %d; parent tgtLeader %d\n", sh, p, H.L.posDrv[p],
+                       H.count[H.L.posDrv[p]], H.ids[p].w, H.nav[p].x, H.leader[p], H.gap[p], H.lcSlot[sh].gap, H.ctrl.nAct[V.par], H.lcSlot[H.shadowLog[k].x].tgtLeader);
                 bool inAct = false;
-                for (int a2 = 0; a2 < H.ctrl.nAct[V.par]; ++a2) inAct |= V.actList[V.par][a2] == H.posDrv[p];
+                for (int a2 = 0; a2 < H.ctrl.nAct[V.par]; ++a2) inAct |= V.actList[V.par][a2] == H.L.posDrv[p];
                 printf("  drivable in actList: %d\n", (int) inAct);
             }
         }
@@ -205,7 +201,7 @@ void compare(Oracle &o, std::vector<Veh *> &removedThisStep) {
         for (auto &kv : o.pool) if (kv.first == want && kv.second->running && slotOf.count(kv.second)) {
             Veh *v = kv.second; const int s = slotOf.at(v); const LcSlot &L = H.lcSlot[s]; const int p = H.pos[s];
             printf("  trace step %zu prio %d: type %d/%d drivable %d/%d dis %.4f/%.4f leader %d/%d own gap %.6f/%.6f V.gap %.6f changing %d/%d\n", o.step, want, v->partnerType, L.type,
-                   v->drivable, H.posDrv[p], v->dis, H.kin[p].x, v->leader ? v->leader->priority : 0, H.leader[p] >= 0 ? H.ids[H.leader[p]].z : 0, v->gap, L.gap, H.gap[p], v->changing, L.changing);
+                   v->drivable, H.L.posDrv[p], v->dis, H.kin[p].x, v->leader ? v->leader->priority : 0, H.leader[p] >= 0 ? H.ids[H.leader[p]].z : 0, v->gap, L.gap, H.gap[p], v->changing, L.changing);
         }
     }
     CHECK((int) o.activeCount == H.ctrl.active, "active vehicles %zu vs %d", o.activeCount, H.ctrl.active);
@@ -214,7 +210,7 @@ void compare(Oracle &o, std::vector<Veh *> &removedThisStep) {
         if ((int) o.lists[d].size() != H.count[d]) continue;
         int k = 0;
         for (Veh *v : o.lists[d]) {
-            const int p = H.off[d] + k++;
+            const int p = H.L.off[d] + k++;
             const int s = slotOf.count(v) ? slotOf.at(v) : -1;
             CHECK(H.ids[p].x == s, "drivable %d position %d: slot %d, expected %d (prio %d)", d, k - 1, H.ids[p].x, s, v->priority);
             if (H.ids[p].x != s) continue;
@@ -269,7 +265,7 @@ int main(int argc, char **argv) {
     if (!o.load(argv[1])) { fprintf(stderr, "cannot load %s\n", argv[1]); return 2; }
     o.routing->enableLanePlans();
     HostSim H;
-    H.init(o.net, o.interval, o.rlTrafficLight, o.laneChange, o.segStart);
+    H.init(o.net, o.interval, o.rlTrafficLight, o.laneChange);
     S = &H;
     const int steps = atoi(argv[2]);
     std::vector<Veh *> removed;

@@ -35,6 +35,7 @@ namespace cfb { namespace cg = cooperative_groups; }
 #include "device_view.cuh"
 #include "device_phases_a.cuh"   // headSearch (the warp code in there is not run by this probe)
 #include "device_control.cuh"   // canPass, phase_control (+ device_lc.cuh)
+#include "device_layout.cuh"    // the product's static tables; the buckets (off, posDrv) are this probe's own
 
 #include "../oracle/cityflow_oracle.cpp"   // Oracle / Veh (anonymous namespace: visible in this translation unit)
 
@@ -43,11 +44,10 @@ namespace {
 using namespace cfb;
 
 struct Soa {   // the arrays the device functions touch, sized for this step
-    std::vector<int> off, count, pos, leader, laneOutBeg, laneOutLinks, planBeg, planData, segIdx, posDrv, segBeg,
-        laneIdx, laneRoadN, planRoute, planRoadPos, lpRoad, lpBeg, lpId, cand, involved, spare, act[2], blk, extra, entCnt, ent;
-    std::vector<double> drvLength, gap, cust, segStart, laneWidth, drvMaxSpeed, lcDist;
-    std::vector<int> llCrossBeg, lcIdx, csLink, delStep, llStartLane, routeLast, laneRoadT;
-    std::vector<int4> linkInfo;
+    std::vector<int> off, count, pos, leader, segIdx, posDrv, cand, involved, spare, act[2], blk, extra, entCnt, ent, delStep;
+    std::vector<double> gap, cust;
+    PlanTables plans;
+    LanePlanTables lanePlans;
     std::vector<unsigned> foeMask;
     std::vector<Notify> notify;
     std::vector<unsigned char> rlAvail;
@@ -69,6 +69,8 @@ struct Soa {   // the arrays the device functions touch, sized for this step
 };
 
 Soa *g = nullptr;
+DeviceLayout g_layout;   // deviceLayout() of the restatement's road network ...
+View g_sized;            // ... and the View sizes it sets
 static int slotAt(Soa &S, Veh *v, const char *what) {
     auto it = S.slotOf.find(v);
     if (it == S.slotOf.end()) { printf("PROBE: %s refers to a vehicle that is not running (prio %d, running %d)\n", what, v->priority, (int) v->running); fflush(stdout); abort(); }
@@ -90,6 +92,7 @@ void build(Oracle &o, bool forControl) {
     g = new Soa();
     Soa &S = *g;
     const RoadNet &net = o.net;
+    const DeviceLayout &L = g_layout;
     const int nL = net.nLanes(), nD = net.nDrivables();
     S.epoch = (int) o.step + 1;
     // buckets: list size + headroom
@@ -100,21 +103,6 @@ void build(Oracle &o, bool forControl) {
     S.kin.assign(P, make_double2(0, 0)); S.ids.assign(P, make_int4(0, 0, 0, 0)); S.nav.assign(P, make_int4(0, 0, 0, 0));
     S.gap.assign(P, 0); S.cust.assign(P, 0); S.segIdx.assign(P, 0); S.leader.assign(P, -1); S.posDrv.assign(P, 0);
     for (int d = 0; d < nD; ++d) for (int p = S.off[d]; p < S.off[d + 1]; ++p) S.posDrv[p] = d;
-    S.drvLength.resize(nD);
-    for (int d = 0; d < nD; ++d) S.drvLength[d] = o.drvLength(d);
-    S.laneOutBeg.assign(nL + 1, 0);
-    for (int l = 0; l < nL; ++l) {
-        S.laneOutBeg[l + 1] = S.laneOutBeg[l] + (int) net.laneOutLinks[l].size();
-        for (int ll : net.laneOutLinks[l]) S.laneOutLinks.push_back(ll);
-    }
-    // static lane tables + segments exactly like DeviceSim::enableLaneChange
-    S.segBeg.assign(nL + 1, 0); S.laneIdx.resize(nL); S.laneRoadN.resize(nL); S.laneWidth.resize(nL);
-    for (int l = 0; l < nL; ++l) {
-        S.segBeg[l] = (int) S.segStart.size();
-        for (double x : o.segStart[l]) S.segStart.push_back(x);
-        S.laneIdx[l] = net.laneIdx[l]; S.laneRoadN[l] = net.roadNumLanes(net.laneRoad[l]); S.laneWidth[l] = net.laneWidth[l];
-    }
-    S.segBeg[nL] = (int) S.segStart.size();
     // slots and per-vehicle records
     int nSlots = 0;
     for (auto &kv : o.pool) if (kv.second->running) { S.slotOf[kv.second] = nSlots++; S.vehOfSlot.push_back(kv.second); }
@@ -152,13 +140,7 @@ void build(Oracle &o, bool forControl) {
             S.gap[p] = v->gap;
             S.cust[p] = v->bCustomSet ? v->bCustom : NAN;
             S.pos[s] = p;
-            DTmpl t{};   // toDevice() of device_sim.cu
-            t.len = v->t.len; t.maxPosAcc = v->t.maxPosAcc; t.maxNegAcc = v->t.maxNegAcc; t.usualPosAcc = v->t.usualPosAcc;
-            t.usualNegAcc = v->t.usualNegAcc; t.minGap = v->t.minGap; t.maxSpeed = v->t.maxSpeed; t.headwayTime = v->t.headwayTime;
-            t.yieldDistance = v->t.yieldDistance; t.turnSpeed = v->t.turnSpeed;
-            t.approachDist = v->t.maxSpeed * v->t.maxSpeed / v->t.usualNegAcc / 2 + v->t.maxSpeed * o.interval * 2;
-            t.speed0 = v->t.speed;
-            S.tmpl[s] = t;
+            S.tmpl[s] = toDevice(v->t, o.interval);
             S.allVeh.push_back(v);
             LcSlot &L = S.slot[s];
             lcResetSlot(L, plan);
@@ -174,12 +156,8 @@ void build(Oracle &o, bool forControl) {
         }
         S.count[d] = k;
     }
-    S.planBeg = R.planBeg(); S.planData = R.planData();
-    S.planRoute = R.planRouteTable(); S.planRoadPos = R.planRoadPosTable();
-    S.lpRoad = R.lanePlanRoadTable(); S.lpBeg = R.lanePlanBegTable(); S.lpId = R.lanePlanIdTable();
-    S.routeLast.assign(std::max(R.numRoutes(), 1), -1);
-    for (int r = 0; r < R.numRoutes(); ++r) if (R.route(r).valid) S.routeLast[r] = R.route(r).roads.back();
-    S.laneRoadT.assign(net.laneRoad.begin(), net.laneRoad.end());
+    S.plans = planTables(R);
+    S.lanePlans = lanePlanTables(R);
     S.tail.resize(nD);
     for (int d = 0; d < nD; ++d) {
         Tail t{}; t.pos = -1; t.prev = -1;
@@ -195,12 +173,11 @@ void build(Oracle &o, bool forControl) {
     S.mkin.assign(8192, make_double2(0, 0)); S.mids.assign(8192, make_int4(0, 0, 0, 0)); S.mnav.assign(8192, make_int4(0, 0, 0, 0));
     S.entCnt.assign(nD, 0); S.ent.assign((size_t) nD * ENT_CAP, 0); S.extra.assign(nD + 8, 0);
     View &V = S.V;
-    V.nLanes = nL; V.nLinks = net.nLinks(); V.nDrv = nD; V.dt = o.interval; V.par = 0; V.vehCap = P + 64;
-    V.drvLength = S.drvLength.data(); V.off = S.off.data(); V.laneOutBeg = S.laneOutBeg.data(); V.laneOutLinks = S.laneOutLinks.data();
-    S.llStartLane.assign(net.llStartLane.begin(), net.llStartLane.end());
-    if (S.llStartLane.empty()) S.llStartLane.push_back(0);
-    V.llStartLane = S.llStartLane.data();   // headSearch (the shadow's immediate leader update)
-    V.tmpl = S.tmpl.data(); V.planBeg = S.planBeg.data(); V.planData = S.planData.data();
+    V = g_sized;
+    V.dt = o.interval; V.par = 0; V.vehCap = P + 64;
+    V.drvLength = L.drvLength.data(); V.off = S.off.data(); V.laneOutBeg = L.laneOutBeg.data(); V.laneOutLinks = L.laneOutLinks.data();
+    V.llStartLane = L.llStartLane.data();   // headSearch (the shadow's immediate leader update)
+    V.tmpl = S.tmpl.data(); V.planBeg = S.plans.planBeg.data(); V.planData = S.plans.planData.data();
     V.kin = S.kin.data(); V.gap = S.gap.data(); V.leader = S.leader.data(); V.ids = S.ids.data(); V.nav = S.nav.data();
     V.count = S.count.data(); V.pos = S.pos.data(); V.tail = S.tail.data(); V.cust = S.cust.data(); V.blk = S.blk.data();
     V.vehList[0] = S.veh[0].data(); V.vehList[1] = S.veh[1].data(); V.actList[0] = S.act[0].data(); V.actList[1] = S.act[1].data();
@@ -210,36 +187,18 @@ void build(Oracle &o, bool forControl) {
     V.entCnt = S.entCnt.data(); V.ent = S.ent.data(); V.extraList = S.extra.data(); V.moverCap = 8192;
     V.lcOn = 1;
     LcView &C = V.lc;
-    C.slot = S.slot.data(); C.segIdx = S.segIdx.data(); C.posDrv = S.posDrv.data(); C.segBeg = S.segBeg.data(); C.segStart = S.segStart.data();
-    C.laneIdx = S.laneIdx.data(); C.laneRoadN = S.laneRoadN.data(); C.laneWidth = S.laneWidth.data();
-    C.planRoute = S.planRoute.data(); C.planRoadPos = S.planRoadPos.data();
-    C.lanePlanRoad = S.lpRoad.data(); C.lanePlanBeg = S.lpBeg.data(); C.lanePlanId = S.lpId.data();
-    C.routeLastRoad = S.routeLast.data(); C.laneRoad = S.laneRoadT.data();
+    C.slot = S.slot.data(); C.segIdx = S.segIdx.data(); C.posDrv = S.posDrv.data(); C.segBeg = L.segBeg.data(); C.segStart = L.segStart.data();
+    C.laneIdx = L.laneIdx.data(); C.laneRoadN = L.laneRoadN.data(); C.laneWidth = L.laneWidth.data();
+    C.planRoute = S.lanePlans.planRoute.data(); C.planRoadPos = S.lanePlans.planRoadPos.data();
+    C.lanePlanRoad = S.lanePlans.lanePlanRoad.data(); C.lanePlanBeg = S.lanePlans.lanePlanBeg.data(); C.lanePlanId = S.lanePlans.lanePlanId.data();
+    C.routeLastRoad = S.lanePlans.routeLastRoad.data(); C.laneRoad = L.laneRoad.data();
     C.cand = S.cand.data(); C.involved = S.involved.data(); C.spare = S.spare.data(); C.nSpare = nSpare;
     C.shadowLog = S.shadowLog.data(); C.ctrl = &S.lcCtrl;
 
-    // ---- what the control phase needs on top (static tables as in DeviceSim::DeviceSim) ----
+    // ---- what the control phase needs on top ----
     const int nK = net.nLinks();
-    S.drvMaxSpeed.resize(nD);
-    for (int d = 0; d < nD; ++d) S.drvMaxSpeed[d] = d < nL ? net.laneMaxSpeed[d] : 10000.0;
-    S.llCrossBeg.assign(nK + 1, 0);
-    for (int k = 0; k < nK; ++k) {
-        for (const CrossRef &c : net.llCrosses[k]) { S.lcIdx.push_back(c.cross * 2 + c.side); S.lcDist.push_back(net.crossDist[c.side][c.cross]); }
-        S.llCrossBeg[k + 1] = (int) S.lcIdx.size();
-    }
-    S.csLink.assign(std::max(2 * net.nCross(), 1), 0);
-    for (int c = 0; c < net.nCross(); ++c) { S.csLink[2 * c] = net.crossLink[0][c]; S.csLink[2 * c + 1] = net.crossLink[1][c]; }
-    std::vector<int> flatOf(std::max(2 * net.nCross(), 1), 0);
-    int maxCross = 1;
-    for (int k = 0; k < nK; ++k) {
-        maxCross = std::max(maxCross, S.llCrossBeg[k + 1] - S.llCrossBeg[k]);
-        for (int q = S.llCrossBeg[k]; q < S.llCrossBeg[k + 1]; ++q) flatOf[S.lcIdx[q]] = q;
-    }
-    V.maskWords = (maxCross + 31) / 32;
-    S.linkInfo.assign(std::max(nK, 1), make_int4(0, 0, 0, 0));
-    for (int k = 0; k < nK; ++k)
-        S.linkInfo[k] = make_int4(net.llRoadLink[k], net.llEndLane[k], S.llCrossBeg[k], (net.linkIsTurn(k) ? 1 : 0) | (net.rlType[net.llRoadLink[k]] << 8));
-    if (S.lcIdx.empty()) { S.lcIdx.push_back(0); S.lcDist.push_back(0); }
+    std::vector<int> flatOf(std::max(2 * net.nCross(), 1), 0);   // where each cross side sits in the cross lists
+    for (int q = 0; q < L.llCrossBeg[nK]; ++q) flatOf[L.lcIdx[q]] = q;
     // this step's notifications (Cross::notify, engine.cpp:317-372) straight from the restatement
     // (before notifyCross has run they are last step's and may point to vehicles that are gone)
     S.notify.assign(std::max(2 * net.nCross(), 1), Notify{0.0, -1, -1});
@@ -250,8 +209,8 @@ void build(Oracle &o, bool forControl) {
             if (!nv) continue;
             const int cs = 2 * c + side;
             S.notify[cs] = Notify{o.notifyDist[side][c], S.pos[slotAt(S, nv, "notify")], S.epoch};
-            const int foeLink = S.csLink[cs ^ 1];
-            const int bit = flatOf[cs ^ 1] - S.llCrossBeg[foeLink];
+            const int foeLink = L.csLink[cs ^ 1];
+            const int bit = flatOf[cs ^ 1] - L.llCrossBeg[foeLink];
             S.foeMask[(size_t) foeLink * V.maskWords + (bit >> 5)] |= 1u << (bit & 31);
         }
     S.rlAvail.assign(std::max(net.nRoadLinks(), 1), 0);
@@ -270,13 +229,13 @@ void build(Oracle &o, bool forControl) {
     }
     S.ctrl.nVeh[0] = nVeh;
     S.ctrl.nCustom = nCustom;
-    V.drvMaxSpeed = S.drvMaxSpeed.data(); V.linkInfo = S.linkInfo.data(); V.llCrossBeg = S.llCrossBeg.data(); V.lcIdx = S.lcIdx.data();
-    V.lcDist = S.lcDist.data(); V.csLink = S.csLink.data(); V.foeMask = S.foeMask.data(); V.notify = S.notify.data();
-    V.rlAvail = S.rlAvail.data(); V.delStep = S.delStep.data(); V.nCross = net.nCross();
+    V.drvMaxSpeed = L.drvMaxSpeed.data(); V.linkInfo = L.linkInfo.data(); V.llCrossBeg = L.llCrossBeg.data(); V.lcIdx = L.lcIdx.data();
+    V.lcDist = L.lcDist.data(); V.csLink = L.csLink.data(); V.foeMask = S.foeMask.data(); V.notify = S.notify.data();
+    V.rlAvail = S.rlAvail.data(); V.delStep = S.delStep.data();
     V.lcOn = o.laneChange ? 1 : 0;
     // the foe half of Cross::canPass, as k_notify attaches it to every notification (device_control.cuh foeTerms)
     for (int cs = 0; forControl && cs < 2 * net.nCross(); ++cs)
-        if (S.notify[cs].epoch == S.epoch && S.notify[cs].pos >= 0) foeTerms(V, S.notify[cs], S.linkInfo[S.csLink[cs]].w);
+        if (S.notify[cs].epoch == S.epoch && S.notify[cs].pos >= 0) foeTerms(V, S.notify[cs], L.linkInfo[L.csLink[cs]].w);
 }
 
 void before(Oracle &o) {
@@ -448,6 +407,7 @@ int main(int argc, char **argv) {
     Oracle o;
     if (!o.load(argv[1])) { fprintf(stderr, "cannot load %s\n", argv[1]); return 2; }
     o.routing->enableLanePlans();
+    g_layout = deviceLayout(o.net, g_sized);
     o.lcProbe = probe;
     o.deviceForm = true;   // (proven equal to the reference order; gives the hook between the two control passes)
     const int steps = atoi(argv[2]);
