@@ -18,6 +18,7 @@ namespace cfb {
 // allocation is non-empty.
 struct DeviceLayout {
     int P = 0;                       // positions: sum of the bucket capacities
+    double spacing = 2.5;            // the vehicle spacing (length + minGap) the buckets are sized for (bucketSpacing)
     std::vector<int> off;            // per drivable: its bucket [off[d], off[d+1])
     std::vector<double> drvLength, drvMaxSpeed;
     std::vector<int> laneOutBeg, laneOutLinks, llStartLane, llEndLane, llRoadLink;
@@ -33,9 +34,23 @@ struct DeviceLayout {
     std::vector<double> segStart, laneWidth;
 };
 
-// Also sets V's sizes: the element counts, maskWords and the capacities moverCap, finCap and vehCap.
-inline DeviceLayout deviceLayout(const RoadNet &net, View &V) {
+// The spacing the lane buckets are sized for: the smallest length + minGap of the given vehicle templates, but at most
+// 2.5 m (so a fleet of vehicles of 2.5 m and more, such as the grid generator's, gets the same layout whatever its
+// sizes) and at least 0.5 m (a degenerate template must not size the buckets without bound).  Queued vehicles keep
+// about length + minGap apart (admission: tail.dis > tail.len + minGap; car following stops minGap behind the
+// leader), so a bucket of length / spacing + 8 holds a lane filled end to end.  That is a target, not an invariant
+// (Lane::canEnter also admits behind a tail moving at 2 m/s or more): ERR_BUCKET_OVERFLOW stays the backstop.
+inline double bucketSpacing(const std::vector<VehicleTemplate> &templates) {
+    double s = 2.5;
+    for (const VehicleTemplate &t : templates) s = std::min(s, t.len + t.minGap);
+    return std::max(s, 0.5);
+}
+
+// Also sets V's sizes: the element counts, maskWords and the capacities moverCap, finCap and vehCap.  `spacing`:
+// bucketSpacing() of the templates known when the layout is made.
+inline DeviceLayout deviceLayout(const RoadNet &net, View &V, double spacing) {
     DeviceLayout L;
+    L.spacing = spacing;
     const int nL = net.nLanes(), nK = net.nLinks(), nD = nL + nK, nC = net.nCross();
     V.nLanes = nL; V.nLinks = nK; V.nDrv = nD; V.nInter = net.nInter(); V.nRL = net.nRoadLinks(); V.nCross = nC;
     auto nz = [](std::vector<int> v) { if (v.empty()) v.push_back(0); return v; };
@@ -45,8 +60,8 @@ inline DeviceLayout deviceLayout(const RoadNet &net, View &V) {
     for (int d = 0; d < nD; ++d) {
         L.drvLength[d] = d < nL ? net.laneLength[d] : net.llLength[d - nL];
         L.drvMaxSpeed[d] = d < nL ? net.laneMaxSpeed[d] : 10000.0;  // LaneLink::maxSpeed, roadnet.h:456
-        // bucket capacity: room for bumper-to-bumper traffic of 2.5 m vehicles plus slack
-        int cap = (int) (L.drvLength[d] / 2.5) + 8;
+        // bucket capacity: room for bumper-to-bumper traffic of vehicles `spacing` apart plus slack
+        int cap = (int) (L.drvLength[d] / spacing) + 8;
         cap = (cap + 3) & ~3;
         L.off[d + 1] = L.off[d] + cap;
     }

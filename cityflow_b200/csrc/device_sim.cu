@@ -529,7 +529,7 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
     V.rl = opt.rlTrafficLight ? 1 : 0;
 
     // ---- static tables ----
-    I.L = deviceLayout(net, V);
+    I.L = deviceLayout(net, V, cfb::bucketSpacing(templates));
     const DeviceLayout &L = I.L;
     const int nL = V.nLanes, nK = V.nLinks, nD = V.nDrv;
     I.P = L.P;
@@ -1292,6 +1292,8 @@ int DeviceSim::tieCount() {
     readCtrlImpl(impl_->stream, impl_->hCtrl, impl_->V.ctrl);
     return impl_->hCtrl->ties;
 }
+
+double DeviceSim::bucketSpacing() const { return impl_->L.spacing; }
 
 int DeviceSim::errorFlags() {
     if (mirrorCurrent(*impl_)) return impl_->hMirror[2];

@@ -118,8 +118,11 @@ public:
     DeviceSim(const DeviceSim &) = delete;
     DeviceSim &operator=(const DeviceSim &) = delete;
 
-    // Re-upload the (grown) template / plan tables.
+    // Re-upload the (grown) template / plan tables.  A template whose length + minGap is below bucketSpacing() would
+    // not fit the lane buckets: the host engine refuses it before it gets here.
     void uploadTemplates(const std::vector<VehicleTemplate> &templates);
+    // The vehicle spacing (length + minGap) the lane buckets were sized for when the engine was made (device_layout.cuh)
+    double bucketSpacing() const;
     void uploadPlans(const Routing &routing);
     void ensureSlotCapacity(int slots);
 

@@ -59,7 +59,7 @@ struct Ctrl {
 namespace cfb {
 
 constexpr int HEAD_BIT = 0x40000000;   // in vehList[].y: the vehicle is the first of its drivable's list
-constexpr int ENT_CAP = 16;   // entrants staged per drivable per step
+constexpr int ENT_CAP = 16;   // entrants staged per drivable per step (measured at most 6 on tests/edgenet.py's shapes, DESIGN §4)
 constexpr int PLAN_LOOKAHEAD_END = -1;
 constexpr int SPAWN_SMEM = 2048;
 

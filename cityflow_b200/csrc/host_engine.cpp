@@ -154,6 +154,17 @@ public:
 
     static uint64_t key(int flow, int index) { return ((uint64_t) (uint32_t) flow << 32) | (uint32_t) index; }
 
+    // The lane buckets are sized once, from the vehicles known when the engine is made (bucketSpacing,
+    // device_layout.cuh).  A vehicle that packs tighter than that could overflow a bucket: refused, not run.
+    void checkFitsLayout(const VehicleTemplate &t) const {
+        if (!dev || t.len + t.minGap >= dev->bucketSpacing()) return;
+        std::ostringstream m;
+        m << "vehicle of length " << t.len << " m with minGap " << t.minGap << " m packs tighter than the lane buckets allow: "
+          << "they were sized for vehicles at least " << dev->bucketSpacing() << " m apart (length + minGap), from the "
+          << "vehicles of the flow file; give the flow file a vehicle this small to run it";
+        throw std::runtime_error(m.str());
+    }
+
     int internTemplate(const VehicleTemplate &t) {
         auto it = templateIndex.find(t);
         if (it != templateIndex.end()) return it->second;
@@ -895,6 +906,7 @@ public:
             if (r < (size_t) routing->numRoutes() ? routing->anchorsOf((int) r) != s.routeAnchors[r] : routing->intern(s.routeAnchors[r]) != (int) r)
                 throw std::runtime_error("archive does not match this engine (route table)");
         }
+        for (size_t t = templates.size(); t < s.templates.size(); ++t) checkFitsLayout(s.templates[t]);
         for (size_t t = 0; t < s.templates.size(); ++t) {
             const bool same = t < templates.size() ? (!(templates[t] < s.templates[t]) && !(s.templates[t] < templates[t])) : internTemplate(s.templates[t]) == (int) t;
             if (!same) throw std::runtime_error("archive does not match this engine (vehicle template table)");
@@ -1095,6 +1107,7 @@ public:
             t.usualPosAcc = dbl(v, "usualPosAcc"); t.usualNegAcc = dbl(v, "usualNegAcc"); t.minGap = dbl(v, "minGap");
             t.maxSpeed = dbl(v, "maxSpeed"); t.headwayTime = dbl(v, "headwayTime"); t.yieldDistance = dbl(v, "yieldDistance");
             t.turnSpeed = dbl(v, "turnSpeed");
+            checkFitsLayout(t);
             si.tmplId = internTemplate(t);
             const Json &rj = member(v, "route");
             if (!rj.isArray()) throw std::runtime_error("route: expected an array");
@@ -1546,6 +1559,7 @@ int cfb_push_vehicle(cfb_engine *e, const double v[10], const char *const *roads
         double *f[10] = {&t.speed, &t.len, &t.width, &t.maxPosAcc, &t.maxNegAcc, &t.usualPosAcc, &t.usualNegAcc,
                          &t.minGap, &t.maxSpeed, &t.headwayTime};
         for (int k = 0; k < 10; ++k) if (!std::isnan(v[k])) *f[k] = v[k];
+        h.checkFitsLayout(t);
         std::vector<int> anchors;
         for (int k = 0; k < n_roads; ++k) {
             auto it = h.net.roadIndex.find(roads[k]);

@@ -144,6 +144,7 @@ struct Oracle {
     std::vector<std::vector<double>> segStart;            // [lane][segment] startPos
     std::vector<std::vector<std::vector<Veh *>>> segVeh;  // [lane][segment] vehicles, list order
     int ties = 0;  // pushBuffer ties (same target drivable, equal dis): order unspecified in the reference
+    int maxRefusedCross = -1;  // highest index in its laneLink's cross list at which Cross::canPass refused a vehicle
     cfb::Routing *routing = nullptr;
 
     int nLanes() const { return net.nLanes(); }
@@ -339,10 +340,12 @@ struct Oracle {
         }
         if (ll < 0 && isLink(v.drivable)) ll = v.drivable - nLanes();
         double distanceToLaneLinkStart = !isLink(v.drivable) ? -(drvLength(v.drivable) - v.dis) : v.dis;
-        for (const cfb::CrossRef &cr : net.llCrosses[ll]) {
+        for (size_t ci = 0; ci < net.llCrosses[ll].size(); ++ci) {
+            const cfb::CrossRef &cr = net.llCrosses[ll][ci];
             double distanceOnLaneLink = net.crossDist[cr.side][cr.cross];
             if (distanceOnLaneLink < distanceToLaneLinkStart) continue;
             if (!canPass(cr.cross, v, ll, distanceToLaneLinkStart)) {
+                maxRefusedCross = std::max(maxRefusedCross, (int) ci);
                 s = min2(s, stopBeforeSpeed(v, distanceOnLaneLink - distanceToLaneLinkStart - v.t.yieldDistance));
                 v.bBlocker = notifyVeh[1 - cr.side][cr.cross];  // setBlocker(getFoeVehicle)
                 v.bBlockerSet = true;
@@ -1175,6 +1178,7 @@ int cfo_pool_size(void *h) { return (int) ((Oracle *) h)->pool.size(); }
 int cfo_finished_count(void *h) { return ((Oracle *) h)->finishedCnt; }
 double cfo_cumulative_travel_time(void *h) { return ((Oracle *) h)->cumulativeTravelTime; }
 int cfo_tie_count(void *h) { return ((Oracle *) h)->ties; }
+int cfo_max_refused_cross_index(void *h) { return ((Oracle *) h)->maxRefusedCross; }
 double cfo_current_time(void *h) { return ((Oracle *) h)->currentTime(); }
 void cfo_lane_vehicle_count(void *h, int32_t *out) {  // engine.cpp:628-634
     Oracle *o = (Oracle *) h;

@@ -369,6 +369,12 @@ class PortOracle:
     def tie_count(self) -> int:
         return self.lib.cfo_tie_count(self.h)
 
+    def max_refused_cross_index(self) -> int:
+        """Highest position in its laneLink's cross list at which Cross::canPass has refused a vehicle so far (-1: none)."""
+        self.lib.cfo_max_refused_cross_index.restype = ctypes.c_int
+        self.lib.cfo_max_refused_cross_index.argtypes = [ctypes.c_void_p]
+        return self.lib.cfo_max_refused_cross_index(self.h)
+
     def _lane_array(self, fn, n=None):
         a = np.zeros(n or self.n_lanes, np.int32)
         getattr(self.lib, fn)(self.h, a.ctypes.data)

@@ -53,8 +53,8 @@ struct HostSim {   // DeviceSim's arrays on the host: the static tables of devic
     LcCtrl lcCtrl{};
     long long steps = 0;
 
-    void init(const RoadNet &net, double interval, bool rl, bool laneChange) {
-        L = deviceLayout(net, V);
+    void init(const RoadNet &net, double interval, bool rl, bool laneChange, double spacing) {
+        L = deviceLayout(net, V, spacing);
         const int nL = V.nLanes, nK = V.nLinks, nD = V.nDrv;
         V.dt = interval; V.rl = rl ? 1 : 0;
         P = L.P;

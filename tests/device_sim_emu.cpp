@@ -67,7 +67,7 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
     }
     Impl &I = *impl_;
     I.opt = opt;
-    I.H.init(net, opt.interval, opt.rlTrafficLight, false);
+    I.H.init(net, opt.interval, opt.rlTrafficLight, false, cfb::bucketSpacing(templates));
     uploadTemplates(templates);
     uploadPlans(routing);
     reset();
@@ -178,6 +178,7 @@ void DeviceSim::synchronize() {}
 
 int DeviceSim::vehicleCount() { return impl_->H.ctrl.active; }
 int DeviceSim::errorFlags() { return impl_->H.ctrl.error; }
+double DeviceSim::bucketSpacing() const { return impl_->H.L.spacing; }
 int DeviceSim::tieCount() { return impl_->H.ctrl.ties; }
 void DeviceSim::laneVehicleCount(int32_t *out) { for (int l = 0; l < impl_->H.V.nLanes; ++l) out[l] = impl_->H.count[l]; }
 void DeviceSim::laneWaitingVehicleCount(int32_t *out) {

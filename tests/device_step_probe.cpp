@@ -265,7 +265,9 @@ int main(int argc, char **argv) {
     if (!o.load(argv[1])) { fprintf(stderr, "cannot load %s\n", argv[1]); return 2; }
     o.routing->enableLanePlans();
     HostSim H;
-    H.init(o.net, o.interval, o.rlTrafficLight, o.laneChange);
+    std::vector<cfb::VehicleTemplate> fleet;
+    for (const auto &f : o.flows) fleet.push_back(f.def.tmpl);
+    H.init(o.net, o.interval, o.rlTrafficLight, o.laneChange, cfb::bucketSpacing(fleet));
     S = &H;
     const int steps = atoi(argv[2]);
     std::vector<Veh *> removed;

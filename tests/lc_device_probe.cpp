@@ -407,7 +407,9 @@ int main(int argc, char **argv) {
     Oracle o;
     if (!o.load(argv[1])) { fprintf(stderr, "cannot load %s\n", argv[1]); return 2; }
     o.routing->enableLanePlans();
-    g_layout = deviceLayout(o.net, g_sized);
+    std::vector<cfb::VehicleTemplate> fleet;
+    for (const auto &f : o.flows) fleet.push_back(f.def.tmpl);
+    g_layout = deviceLayout(o.net, g_sized, cfb::bucketSpacing(fleet));
     o.lcProbe = probe;
     o.deviceForm = true;   // (proven equal to the reference order; gives the hook between the two control passes)
     const int steps = atoi(argv[2]);

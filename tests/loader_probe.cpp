@@ -21,6 +21,16 @@ int main(int argc, char **argv) {
                    n.crossDist[c.side][c.cross], n.crossDist[1 - c.side][c.cross]);
             first = false;
         }
+    printf("], \"lane_out\": [");
+    for (int l = 0; l < n.nLanes(); ++l) {
+        printf("%s[", l ? "," : "");
+        for (size_t j = 0; j < n.laneOutLinks[l].size(); ++j) printf("%s%d", j ? "," : "", n.laneOutLinks[l][j]);
+        printf("]");
+    }
+    printf("], \"link_end\": [");
+    for (int k = 0; k < n.nLinks(); ++k) printf("%s%d", k ? "," : "", n.llEndLane[k]);
+    printf("], \"link_cross_count\": [");
+    for (int k = 0; k < n.nLinks(); ++k) printf("%s%d", k ? "," : "", (int) n.llCrosses[k].size());
     printf("]}\n");
     return 0;
 }

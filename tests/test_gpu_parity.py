@@ -636,3 +636,103 @@ def test_30x30_through_the_bench_window_vs_compiled_reference(scenario_dir):
 def test_6x6_3600_steps_vs_port(cfg_6x6):
     """BASELINE.json configs[1] length: the generator's default 6x6 scenario for the full 3600 steps, full state every 100."""
     _run_against_port(cfg_6x6, 3600, every=100)
+
+
+# ------------------------------------------------------------------------------------------
+# Edge shapes (tests/edgenet.py): buckets of 3+ warp chunks filled beyond 2.5 m spacing, laneLinks with more than 32
+# vehicles and more than 64 crosses (three mask words and more), vehicles crossing 3+ drivables per step.  The restatement
+# is pinned to the compiled reference on the same shapes (tests/test_cpu.py::test_edge_network_loader_and_restatement_vs_reference).
+def _edge_static(cfg):
+    import edgenet
+    return edgenet.loader_tables(cfg)
+
+
+@pytest.mark.parametrize("shape,steps", [("long_queue", 700), ("star", 400), ("short_hops", 500)])
+def test_edge_networks_vs_port(shape, steps, tmp_path):
+    import edgenet
+    cfg = edgenet.write(shape, str(tmp_path))
+    static = _edge_static(cfg)
+    reach = edgenet.Reach(static)
+    eng, ora = _run_against_port(cfg, steps, hook=lambda eng, ora, s: reach.add(eng.debug_vehicles()))
+    print("%s: %s; highest refused cross index %d" % (shape, reach, ora.max_refused_cross_index()))
+    assert ora.tie_count() == 0 and eng.average_travel_time() == ora.average_travel_time()
+    if shape == "long_queue":
+        assert reach.lane_occ > 96 and reach.link_occ > 32
+    if shape == "star":
+        assert max(static["link_cross_count"]) > 64 and ora.max_refused_cross_index() >= 32
+    if shape == "short_hops":
+        assert reach.hops >= 3
+
+
+def test_edge_long_queue_lane_change_vs_restatement(tmp_path):
+    """Lane change over buckets of 3+ warp chunks (shadow inserts into long buckets, segment scans): every running
+    vehicle including shadows, every field, every step."""
+    import ctypes
+    import edgenet
+    from cityflow_b200.capi import CEngine
+    cfg = edgenet.write("long_queue", str(tmp_path), lane_change=True)
+    eng, ora = CEngine(cfg), H.PortOracle(cfg)
+    lib = eng.lib
+    lib.cfb_debug_lc_vehicles.restype = ctypes.c_int64
+    lib.cfb_debug_lc_vehicles.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64]
+    reach = edgenet.Reach(_edge_static(cfg))
+    shadows = 0
+    for s in range(1, 701):
+        eng.next_step()
+        ora.next_step()
+        want = ora.lc_snapshot()
+        n = int(lib.cfb_debug_lc_vehicles(eng.h, None, 0))
+        got = np.zeros(n, H.LC_DTYPE)
+        if n:
+            lib.cfb_debug_lc_vehicles(eng.h, got.ctypes.data, n)
+        assert eng.vehicle_count() == want.vehicle_count, "step %d" % s
+        assert np.array_equal(eng.lane_vehicle_count(), want.lane_count), "lane counts, step %d" % s
+        assert len(got) == len(want.vehicles), "step %d" % s
+        for f in H.LC_DTYPE.names:
+            assert np.array_equal(got[f], want.vehicles[f]), "step %d field %s" % (s, f)
+        shadows += int((want.vehicles["partner_type"] == 2).sum())
+        reach.add(got[got["partner_type"] != 2])
+    print("long_queue with lane change: %s; %d shadow states" % (reach, shadows))
+    assert shadows > 100 and reach.lane_occ > 96 and reach.link_occ > 32
+
+
+def test_edge_star_vs_compiled_reference(tmp_path):
+    """laneLinks with hundreds of crosses straight against the UNMODIFIED reference: the cross order of the product's
+    loader cannot hide behind the restatement, which shares it."""
+    if not H.have_ref():
+        pytest.skip("oracle/_ref was not built")
+    import edgenet
+    from cityflow_b200.capi import CEngine
+    cfg = edgenet.write("star", str(tmp_path))
+    eng = CEngine(cfg)
+    ref = H.RefDump.run(cfg, 400, threads=1, every=1, n_inter=eng.n_inter, n_drivables=eng.n_drivables)
+    for st in ref:
+        eng.next_step()
+        bad = H.compare_states(_relax(st), _gpu_state(eng, st.step), check_order=False)
+        assert not bad, "step %d: %s" % (st.step, "; ".join(bad[:6]))
+    assert eng.tie_count() == 0 and ref[-1].vehicle_count > 1000
+
+
+def test_edge_long_queue_lane_observations(tmp_path):
+    """LaneObservations (per-lane warp loops over buckets of more than 64 vehicles) against the host getters."""
+    import cityflow
+    import cityflow_b200
+    import edgenet
+    cfg = edgenet.write("long_queue", str(tmp_path))
+    eng = cityflow.Engine(cfg, thread_num=1)
+    obs = cityflow_b200.LaneObservations(eng)
+    most = 0
+    for _ in range(7):
+        eng.next_steps(100)
+        obs.refresh()
+        counts, waiting = eng.get_lane_vehicle_count(), eng.get_lane_waiting_vehicle_count()
+        assert obs.vehicle_count.tolist() == [counts[i] for i in obs.lane_ids]
+        assert obs.waiting_count.tolist() == [waiting[i] for i in obs.lane_ids]
+        speeds = eng.get_vehicle_speed()
+        per_lane = {i: 0.0 for i in obs.lane_ids}
+        for lane, vs in eng.get_lane_vehicles().items():
+            per_lane[lane] = sum(speeds[v] for v in vs)
+        np.testing.assert_allclose(obs.speed_sum.cpu().numpy(), np.array([per_lane[i] for i in obs.lane_ids]), rtol=0, atol=1e-9)
+        most = max(most, max(counts.values()))
+    print("long_queue: most vehicles on one lane %d" % most)
+    assert most > 96
