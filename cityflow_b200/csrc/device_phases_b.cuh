@@ -112,7 +112,8 @@ __device__ __forceinline__ void phase_move(const View &V, const int bid, const i
                 const double od = __shfl_sync(0xffffffffu, myDis, j);
                 const int op = __shfl_sync(0xffffffffu, myPrio, j);
                 if (lane < m && j != lane && (od > myDis || (od == myDis && op < myPrio))) ++rank;
-                if (lane < m && j < lane && od == myDis) atomicAdd(&V.ctrl->ties, 1);   // (never in the tested scenarios up to 30x30)
+                // each same-distance pair once; the rank above orders it by priority (tests/edgenet.py merge_ties)
+                if (lane < m && j < lane && od == myDis) atomicAdd(&V.ctrl->ties, 1);
             }
             double pd = carryDis, pl = carryLen;                   // list predecessor of the first entrant: the last survivor
             for (int j = 0; j < m; ++j) {

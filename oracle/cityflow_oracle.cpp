@@ -144,6 +144,15 @@ struct Oracle {
     std::vector<std::vector<double>> segStart;            // [lane][segment] startPos
     std::vector<std::vector<std::vector<Veh *>>> segVeh;  // [lane][segment] vehicles, list order
     int ties = 0;  // pushBuffer ties (same target drivable, equal dis): order unspecified in the reference
+    // what a run reached around the tie rule (tests/test_cpu.py prints and asserts these)
+    std::vector<int> tieGroups;  // [k]: steps x drivables where k pushBuffer entries had one target drivable and one distance
+    int tiesBehindSurvivors = 0;  // tied pairs into a drivable that still held vehicles from the step before
+    int maxMovers = 0;          // largest pushBuffer of one step
+    // lane change: searches of a neighbour lane (estimateGap in makeSignal, targetLeader / targetFollower in
+    // scheduling) that found a vehicle at the searcher's bit-equal distance there, and shadows inserted into a lane
+    // holding a vehicle at the parent's bit-equal distance
+    mutable long long lcEqualDisEstimates = 0;
+    long long lcEqualDisSchedules = 0, lcEqualDisInsertions = 0;
     int maxRefusedCross = -1;  // highest index in its laneLink's cross list at which Cross::canPass refused a vehicle
     cfb::Routing *routing = nullptr;
 
@@ -445,8 +454,14 @@ struct Oracle {
                 if ((*it)->dis >= dis) return *it;
         return nullptr;
     }
+    bool holdsDistance(int lane, double dis) const {
+        for (Veh *x : lists[lane])
+            if (x->dis == dis) return true;
+        return false;
+    }
     // SimpleLaneChange::estimateGap lanechange.cpp:220-225
     double estimateGap(const Veh &v, int lane) const {
+        if (holdsDistance(lane, v.dis)) ++lcEqualDisEstimates;
         Veh *leader = vehicleAfter(lane, v.dis, v.segIndex);
         if (!leader) return net.laneLength[lane] - v.dis;
         return leader->dis - v.dis - leader->t.len;
@@ -493,6 +508,7 @@ struct Oracle {
     void updateLeaderAndFollower(Veh &v) {
         v.targetLeader = v.targetFollower = nullptr;
         const int target = v.sigSend->target;
+        if (holdsDistance(target, v.dis)) ++lcEqualDisSchedules;
         v.targetLeader = vehicleAfter(target, v.dis, v.segIndex);
         const int cur = v.drivable;
         v.leaderGap = v.followerGap = std::numeric_limits<double>::max();
@@ -583,6 +599,7 @@ struct Oracle {
         sh->blocker = nullptr;
         sh->drivable = target;
         routerUpdate(*sh);
+        if (holdsDistance(target, v.dis)) ++lcEqualDisInsertions;
         auto &L = lists[target];
         auto pos = L.end();
         if (v.targetFollower) {  // targetFollower->getListIterator(): looked up through ITS segment (vehicle.cpp:404-411)
@@ -676,7 +693,7 @@ struct Oracle {
     // Device form of threadGetAction: pass 1 in arbitrary (here: descending priority) order computes
     // what does not depend on the order; pass 2 finishes the plain vehicles in arbitrary order and
     // only the vehicles involved in a lane change (a partner, or a received signal) in ascending
-    // priority, as the reference's single worker does.
+    // priority, as the reference's single worker does.  The movers are then put in priority order.
     void controlDeviceForm() {
         for (auto it = pool.rbegin(); it != pool.rend(); ++it)
             if (it->second->running) it->second->ctlHead = nextSpeedHead(*it->second);
@@ -692,6 +709,12 @@ struct Oracle {
         statMaxInvolved = std::max(statMaxInvolved, (int) involved.size());
         statRunning += (long long) activeCount;
         for (auto it = involved.rbegin(); it != involved.rend(); ++it) vehicleControl(**it);   // ascending priority
+        // The two passes above fill pushBuffer out of priority order.  Its order decides how updateLocation's stable
+        // sort breaks equal distances into one drivable; the reference's single worker fills it in ascending priority,
+        // and k_move ranks equal-distance entrants by ascending priority.  Put it back into that order (priorities of
+        // live vehicles are unique).
+        std::sort(pushBuffer.begin(), pushBuffer.end(),
+                  [](const std::pair<Veh *, double> &a, const std::pair<Veh *, double> &b) { return a.first->priority < b.first->priority; });
         if (lcProbe) lcProbe(*this, 3);
     }
     // LaneChange::finishChanging lanechange.cpp:115-127 + Vehicle::finishChanging vehicle.cpp:378-381
@@ -974,10 +997,26 @@ struct Oracle {
             L.resize(w);
         }
         // tie order inside std::sort is unspecified in the reference; here: stable, pool order
+        maxMovers = std::max(maxMovers, (int) pushBuffer.size());
+        for (size_t a = 0; a < pushBuffer.size(); ++a) {
+            int group = 1;
+            bool first = true;
+            for (size_t b = 0; b < pushBuffer.size(); ++b)
+                if (b != a && pushBuffer[a].second == pushBuffer[b].second && pushBuffer[a].first->bDrv == pushBuffer[b].first->bDrv) {
+                    ++group;
+                    first &= b > a;
+                }
+            if (group > 1 && first) {   // each group once, at its first member
+                if ((int) tieGroups.size() <= group) tieGroups.resize(group + 1, 0);
+                ++tieGroups[group];
+            }
+        }
         for (size_t a = 0; a + 1 < pushBuffer.size(); ++a)
             for (size_t b = a + 1; b < pushBuffer.size(); ++b)
                 if (pushBuffer[a].second == pushBuffer[b].second && pushBuffer[a].first->bDrv == pushBuffer[b].first->bDrv) {
                     ++ties;
+                    const int d = pushBuffer[a].first->bDrv;
+                    if (d >= 0 && !lists[d].empty()) ++tiesBehindSurvivors;   // the survivors are compacted above
                     if (getenv("CFO_PRINT_TIES"))
                         fprintf(stderr, "[oracle] tie at step %zu: drivable %d dis %.17g  flow_%d_%d (from %d, speed %.17g) vs flow_%d_%d (from %d, speed %.17g)\n", step,
                                 pushBuffer[a].first->bDrv, pushBuffer[a].second, pushBuffer[a].first->flow, pushBuffer[a].first->cnt, pushBuffer[a].first->drivable, pushBuffer[a].first->bSpeed,
@@ -1179,6 +1218,15 @@ int cfo_finished_count(void *h) { return ((Oracle *) h)->finishedCnt; }
 double cfo_cumulative_travel_time(void *h) { return ((Oracle *) h)->cumulativeTravelTime; }
 int cfo_tie_count(void *h) { return ((Oracle *) h)->ties; }
 int cfo_max_refused_cross_index(void *h) { return ((Oracle *) h)->maxRefusedCross; }
+int cfo_tie_groups_of_size(void *h, int k) {
+    const auto &g = ((Oracle *) h)->tieGroups;
+    return k >= 0 && k < (int) g.size() ? g[k] : 0;
+}
+int cfo_ties_behind_survivors(void *h) { return ((Oracle *) h)->tiesBehindSurvivors; }
+int cfo_max_movers(void *h) { return ((Oracle *) h)->maxMovers; }
+long long cfo_lc_equal_distance_estimates(void *h) { return ((Oracle *) h)->lcEqualDisEstimates; }
+long long cfo_lc_equal_distance_schedules(void *h) { return ((Oracle *) h)->lcEqualDisSchedules; }
+long long cfo_lc_equal_distance_insertions(void *h) { return ((Oracle *) h)->lcEqualDisInsertions; }
 double cfo_current_time(void *h) { return ((Oracle *) h)->currentTime(); }
 void cfo_lane_vehicle_count(void *h, int32_t *out) {  // engine.cpp:628-634
     Oracle *o = (Oracle *) h;

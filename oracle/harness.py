@@ -234,9 +234,13 @@ class RefDump:
             return parse_static(f.name)
 
     @staticmethod
-    def run(config: str, steps: int, threads: int = 1, every: int = 1, *, n_inter: int, n_drivables: int):
+    def run(config: str, steps: int, threads: int = 1, every: int = 1, *, n_inter: int, n_drivables: int, patched: bool = False):
+        """`patched`: the priority-ordered build (oracle/lc_order_patch.sh).  At one thread it fills pushBuffer in
+        ascending priority, and libstdc++'s std::sort of at most 16 elements is an insertion sort, so up to 16 movers
+        per step it breaks same-distance ties by ascending priority."""
         with tempfile.NamedTemporaryFile(suffix=".bin") as f:
-            subprocess.check_call([REFDUMP, "run", config, str(steps), str(threads), f.name, str(every)], timeout=REF_TIMEOUT)
+            subprocess.check_call([REFDUMP_LC if patched else REFDUMP, "run", config, str(steps), str(threads), f.name, str(every)],
+                                  timeout=REF_TIMEOUT)
             return parse_run(f.name, n_inter, n_drivables)
 
     @staticmethod
@@ -374,6 +378,26 @@ class PortOracle:
         self.lib.cfo_max_refused_cross_index.restype = ctypes.c_int
         self.lib.cfo_max_refused_cross_index.argtypes = [ctypes.c_void_p]
         return self.lib.cfo_max_refused_cross_index(self.h)
+
+    def tie_reach(self) -> dict:
+        """What the run so far reached around the tie rule: tied pairs, the largest tie group, tied pairs into a
+        drivable that held survivors, the largest number of movers in one step, and (lane change) neighbour-lane
+        searches and shadow insertions that met a vehicle at exactly the searcher's distance."""
+        out = {"ties": self.tie_count()}
+        self.lib.cfo_tie_groups_of_size.restype = ctypes.c_int
+        self.lib.cfo_tie_groups_of_size.argtypes = [ctypes.c_void_p, ctypes.c_int]
+        out["groups"] = {k: n for k in range(2, 33) for n in [self.lib.cfo_tie_groups_of_size(self.h, k)] if n}
+        out["max_group"] = max(out["groups"], default=0)
+        for key, name, typ in (("behind_survivors", "cfo_ties_behind_survivors", ctypes.c_int),
+                               ("max_movers", "cfo_max_movers", ctypes.c_int),
+                               ("lc_equal_estimates", "cfo_lc_equal_distance_estimates", ctypes.c_longlong),
+                               ("lc_equal_schedules", "cfo_lc_equal_distance_schedules", ctypes.c_longlong),
+                               ("lc_equal_insertions", "cfo_lc_equal_distance_insertions", ctypes.c_longlong)):
+            fn = getattr(self.lib, name)
+            fn.restype = typ
+            fn.argtypes = [ctypes.c_void_p]
+            out[key] = int(fn(self.h))
+        return out
 
     def _lane_array(self, fn, n=None):
         a = np.zeros(n or self.n_lanes, np.int32)

@@ -205,6 +205,7 @@ void compare(Oracle &o, std::vector<Veh *> &removedThisStep) {
         }
     }
     CHECK((int) o.activeCount == H.ctrl.active, "active vehicles %zu vs %d", o.activeCount, H.ctrl.active);
+    CHECK(o.ties == H.ctrl.ties, "same-distance entrant pairs so far: restatement %d, device %d", o.ties, H.ctrl.ties);
     for (int d = 0; d < V.nDrv; ++d) {
         CHECK((int) o.lists[d].size() == H.count[d], "drivable %d holds %zu vs %d vehicles", d, o.lists[d].size(), H.count[d]);
         if ((int) o.lists[d].size() != H.count[d]) continue;
@@ -276,6 +277,7 @@ int main(int argc, char **argv) {
         deviceStep(o);
         compare(o, removed);
     }
-    printf("%s %lld steps, %lld vehicle states, %lld finished, %lld shadows, %d failures\n", g_fail ? "FAIL" : "OK", H.steps, g_checked, g_finished, g_shadows, g_fail);
+    printf("%s %lld steps, %lld vehicle states, %lld finished, %lld shadows, %d failures, %d ties\n", g_fail ? "FAIL" : "OK", H.steps, g_checked, g_finished,
+           g_shadows, g_fail, H.ctrl.ties);
     return g_fail ? 1 : 0;
 }

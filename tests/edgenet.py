@@ -12,9 +12,17 @@ fixed capacity that the grid generator and tests/randnet.py never reach:
   step: vehicles crossing 3 or more drivables in one step, leader searches over many drivables, and several
   entrants per lane per step.
 
-Every flow has its own vehicle parameters (as scenario.random_walk_flows' fleet_spread does), so that two entrants
-never tie and the unmodified reference's result is defined; flow intervals are at least 1 s (flow.h:34 asserts it).
-The fixed-time plans hold the approaches red, not rlTrafficLight: the unmodified reference is run from the JSON alone.
+* ``merge_ties`` -- the opposite: parallel, bit-equal approaches whose flows share one vehicle template per group and
+  run in lockstep, so that 2, 3 and 4 vehicles enter one lane in the same step at the same distance, on an empty
+  lane and behind survivors, and (two target lanes) vehicles on neighbouring lanes share a distance.  It exercises
+  the tie rule: same-step entrants with equal distance are ordered by ascending priority.
+
+In the first three shapes every flow has its own vehicle parameters (as scenario.random_walk_flows' fleet_spread
+does), so that two entrants never tie and the unmodified reference's result is defined.  The unmodified reference
+breaks ties by heap address, so merge_ties is compared with it only up to its first tie, and beyond that with the
+priority-ordered build (oracle/lc_order_patch.sh), whose tie order is ascending priority while at most 16 vehicles
+change drivable per step.  Flow intervals are at least 1 s (flow.h:34 asserts it).  The fixed-time plans hold the
+approaches red, not rlTrafficLight: the unmodified reference is run from the JSON alone.
 
 The ``reach`` helpers measure what a run actually reached, so that a test can assert its edge."""
 import math
@@ -234,7 +242,82 @@ def short_hops(seed: int, rows: int = 4, cols: int = 5):
     return net, flows
 
 
-SHAPES = {"long_queue": (long_queue, 1.0), "star": (star, 1.0), "short_hops": (short_hops, 2.0)}
+MERGE_GROUPS = {"P": (0, 0, 1, 1), "Q": (0, 0, 0), "R": (1, 1, 1, 1)}   # target lane on I -> J of every approach road
+
+
+def merge_ties(seed: int):
+    """(roadnet, flows): single-lane approach roads into one merge intersection I, then a two-lane road I -> J to a
+    second real intersection J and an exit road.  The approach roads are parallel translates of each other along y
+    (lane lengths are then computed from x alone, so they are bit-equal), and so are their laneLinks into I -> J:
+    explicit two-point horizontal polylines of equal x span, so they are parallel, have no crosses, and leave nothing
+    at I that could tell two approaches apart.  One phase releases every movement at I and at J.
+
+    Every merge group of MERGE_GROUPS has one vehicle template and one (interval, startTime) shared by its flows, one
+    flow per approach road: its vehicles run in lockstep and enter their target lane in the same step at the same
+    distance.  P sends a pair into each lane (equal distances on neighbouring lanes), Q three and R four vehicles into
+    one lane.  Two background flows with their own parameters use approaches of their own, one per target lane, so
+    that ties also land behind survivors."""
+    rng = random.Random(seed)
+    w_i, w_j = rng.uniform(10, 14), rng.uniform(8, 12)
+    d_ij, l_app, l_exit = rng.uniform(220, 260), 300.0, 300.0
+    approaches = [("%s%d" % (g, k), t) for g, lanes in sorted(MERGE_GROUPS.items()) for k, t in enumerate(lanes)]
+    approaches += [("B0", 0), ("B1", 1)]
+    inters = {"I": {"id": "n_I", "point": {"x": 0.0, "y": 0.0}, "width": w_i, "roads": [], "roadLinks": [], "virtual": False},
+              "J": {"id": "n_J", "point": {"x": d_ij, "y": 0.0}, "width": w_j, "roads": [], "roadLinks": [], "virtual": False},
+              "X": {"id": "n_X", "point": {"x": d_ij + l_exit, "y": 0.0}, "width": 0, "roads": [], "roadLinks": [], "virtual": True}}
+    lane = lambda: {"width": 3.5, "maxSpeed": 13.89}
+
+    def road(rid, a, b, pa, pb, n):
+        inters[a]["roads"].append(rid)
+        inters[b]["roads"].append(rid)
+        return {"id": rid, "points": [{"x": pa[0], "y": pa[1]}, {"x": pb[0], "y": pb[1]}], "lanes": [lane() for _ in range(n)],
+                "startIntersection": inters[a]["id"], "endIntersection": inters[b]["id"]}
+
+    roads = []
+    for k, (name, target) in enumerate(approaches):
+        y = 12.0 * (k + 1)
+        inters[name] = {"id": "n_%s" % name, "point": {"x": -l_app, "y": y}, "width": 0, "roads": [], "roadLinks": [], "virtual": True}
+        roads.append(road("r_%s__I" % name, name, "I", (-l_app, y), (0.0, y), 1))
+        inters["I"]["roadLinks"].append({"type": "go_straight", "startRoad": "r_%s__I" % name, "endRoad": "r_I__J", "direction": 0,
+                                         "laneLinks": [{"startLaneIndex": 0, "endLaneIndex": target,
+                                                        "points": [{"x": -w_i, "y": y}, {"x": w_i, "y": y}]}]})
+    roads.append(road("r_I__J", "I", "J", (0.0, 0.0), (d_ij, 0.0), 2))
+    roads.append(road("r_J__X", "J", "X", (d_ij, 0.0), (d_ij + l_exit, 0.0), 2))
+    inters["J"]["roadLinks"].append({"type": "go_straight", "startRoad": "r_I__J", "endRoad": "r_J__X", "direction": 0,
+                                     "laneLinks": [{"startLaneIndex": 0, "endLaneIndex": 0}, {"startLaneIndex": 1, "endLaneIndex": 1}]})
+    for inter in inters.values():
+        inter["trafficLight"] = {"roadLinkIndices": [], "lightphases": []}
+        if not inter["virtual"]:
+            _set_phases(inter, [(60, list(range(len(inter["roadLinks"]))))])
+    net = {"intersections": [inters[k] for k in sorted(inters)], "roads": roads}
+    flows = []
+    timing = {"P": (12.0, 0), "Q": (16.0, 4), "R": (20.0, 8)}
+    for g in sorted(MERGE_GROUPS):
+        veh = _vehicle(rng, rng.uniform(4.0, 5.0), rng.uniform(2.0, 2.5), rng.uniform(11.0, 13.0), rng.uniform(1.0, 1.5))
+        interval, start = timing[g]
+        for k in range(len(MERGE_GROUPS[g])):
+            flows.append({"vehicle": dict(veh), "route": ["r_%s%d__I" % (g, k), "r_I__J", "r_J__X"], "interval": interval,
+                          "startTime": start, "endTime": -1})
+    for name in ("B0", "B1"):
+        flows.append({"vehicle": _vehicle(rng, rng.uniform(4.0, 6.0), rng.uniform(2.0, 2.5), rng.uniform(10.0, 14.0), rng.uniform(1.0, 1.5)),
+                      "route": ["r_%s__I" % name, "r_I__J", "r_J__X"], "interval": rng.uniform(15.0, 25.0), "startTime": rng.choice([0, 2]),
+                      "endTime": -1})
+    return net, flows
+
+
+def merge_approach_lanes(cfg: str) -> dict:
+    """{group: lane indices of its approach roads} of a merge_ties config ("B": the background approaches)."""
+    import json
+    c = json.load(open(cfg))
+    lane, out = 0, {}
+    for r in json.load(open(c["dir"] + c["roadnetFile"]))["roads"]:
+        if r["id"].endswith("__I"):
+            out.setdefault(r["id"][2], []).append(lane)
+        lane += len(r["lanes"])
+    return out
+
+
+SHAPES = {"long_queue": (long_queue, 1.0), "star": (star, 1.0), "short_hops": (short_hops, 2.0), "merge_ties": (merge_ties, 1.0)}
 
 
 def write(shape: str, directory: str, seed: int = 1, lane_change: bool = False) -> str:

@@ -736,3 +736,109 @@ def test_edge_long_queue_lane_observations(tmp_path):
         most = max(most, max(counts.values()))
     print("long_queue: most vehicles on one lane %d" % most)
     assert most > 96
+
+
+# ------------------------------------------------------------------------------------------
+# The tie rule (tests/edgenet.py merge_ties): 2, 3 and 4 vehicles enter one lane in the same step at the same distance.
+# k_move ranks them by ascending priority whatever order they were staged in (atomics: nondeterministic).  The
+# restatement's tie order is pinned to the priority-ordered reference on this shape
+# (tests/test_cpu.py::test_tie_rule_restatement_vs_priority_ordered_reference).  The GPU's state has no list positions:
+# list order shows in leader, gap and blocker, which differ for a swapped pair.
+TIE_STEPS = 600
+
+
+def test_tie_network_vs_port_twice(tmp_path):
+    """Two runs on the GPU, each equal to the restatement every step, tie counts included: a tie order that followed
+    the staging order would differ between runs or from the restatement."""
+    import edgenet
+    cfg = edgenet.write("merge_ties", str(tmp_path))
+    for run in range(2):
+        counts = []
+        eng, ora = _run_against_port(cfg, TIE_STEPS, hook=lambda eng, ora, s: counts.append((s, eng.tie_count(), ora.tie_count())))
+        assert eng.tie_count() == ora.tie_count()
+        assert all(a == b for _, a, b in counts), [c for c in counts if c[1] != c[2]][:3]
+        assert eng.average_travel_time() == ora.average_travel_time()
+        print("merge_ties run %d: %d tied pairs" % (run, ora.tie_count()))
+        assert ora.tie_count() >= 50
+
+
+def test_tie_network_lane_change_vs_restatement(tmp_path):
+    """merge_ties with lane change: tied pairs in both lanes of I -> J, neighbours at bit-equal distances, every
+    running vehicle including shadows, every field, every step."""
+    import ctypes
+    import edgenet
+    from cityflow_b200.capi import CEngine
+    cfg = edgenet.write("merge_ties", str(tmp_path), lane_change=True)
+    eng, ora = CEngine(cfg), H.PortOracle(cfg)
+    lib = eng.lib
+    lib.cfb_debug_lc_vehicles.restype = ctypes.c_int64
+    lib.cfb_debug_lc_vehicles.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64]
+    shadows = 0
+    for s in range(1, TIE_STEPS + 1):
+        eng.next_step()
+        ora.next_step()
+        want = ora.lc_snapshot()
+        n = int(lib.cfb_debug_lc_vehicles(eng.h, None, 0))
+        got = np.zeros(n, H.LC_DTYPE)
+        if n:
+            lib.cfb_debug_lc_vehicles(eng.h, got.ctypes.data, n)
+        assert eng.vehicle_count() == want.vehicle_count, "step %d" % s
+        assert np.array_equal(eng.lane_vehicle_count(), want.lane_count), "lane counts, step %d" % s
+        assert len(got) == len(want.vehicles), "step %d" % s
+        for f in H.LC_DTYPE.names:
+            assert np.array_equal(got[f], want.vehicles[f]), "step %d field %s" % (s, f)
+        assert eng.tie_count() == ora.tie_count(), "step %d" % s
+        shadows += int((want.vehicles["partner_type"] == 2).sum())
+    reach = ora.tie_reach()
+    print("merge_ties with lane change: %s; %d shadow states" % (reach, shadows))
+    assert reach["ties"] >= 50 and reach["lc_equal_schedules"] >= 1 and shadows > 0
+
+
+def test_tie_network_sharded_loopback_vs_restatement(tmp_path):
+    """merge_ties on two ranks of one GPU: I on rank 0, J on rank 1, so I -> J is a seam lane and the tied entrants
+    reach its owner through the mover mailbox.  Every vehicle equal to the restatement every step."""
+    import edgenet
+    from cityflow_b200.capi import CShardGroup
+    cfg = edgenet.write("merge_ties", str(tmp_path))
+    grp, ora = CShardGroup(cfg, 2), H.PortOracle(cfg)
+    for s in range(1, TIE_STEPS + 1):
+        grp.next_step()
+        ora.next_step()
+        st = ora.snapshot()
+        assert grp.vehicle_count() == st.vehicle_count, "step %d" % s
+        assert np.array_equal(grp.lane_counts(ora.n_lanes), st.lane_count), "lane counts, step %d" % s
+        a, b = np.sort(grp.debug_vehicles(), order=["flow", "cnt"]), np.sort(st.vehicles, order=["flow", "cnt"])
+        assert len(a) == len(b), "step %d" % s
+        for f in ("flow", "cnt", "priority", "drivable", "dis", "speed", "leader_flow", "leader_cnt", "blocker_flow", "blocker_cnt", "gap",
+                  "enter_ll_time"):
+            assert np.array_equal(a[f], b[f]), "step %d field %s" % (s, f)
+    assert ora.tie_count() >= 50
+
+
+def test_tie_network_binary_snapshot_with_a_tied_pair(tmp_path):
+    """A binary snapshot taken while a tied pair shares a lane at one distance, loaded into a fresh engine and run on
+    for 100 steps against the restatement: the image codec has to keep the pair's list order."""
+    import edgenet
+    from cityflow_b200.capi import CEngine
+    cfg = edgenet.write("merge_ties", str(tmp_path))
+    eng, ora = CEngine(cfg), H.PortOracle(cfg)
+    for s in range(1, 400):
+        eng.next_step()
+        ora.next_step()
+        v = ora.vehicles()
+        if s > 100 and len({(int(d), float(x)) for d, x in zip(v["drivable"], v["dis"])}) < len(v):
+            break
+    else:
+        pytest.fail("no two vehicles shared a drivable and a distance")
+    path = str(tmp_path / "tied.bin")
+    eng.dump(path)
+    fresh = CEngine(cfg)
+    fresh.load_from_file(path)
+    bad = H.compare_states(_relax(ora.snapshot()), _gpu_state(fresh, s))
+    assert not bad, "after load at step %d: %s" % (s, "; ".join(bad[:6]))
+    for k in range(1, 101):
+        fresh.next_step()
+        ora.next_step()
+        bad = H.compare_states(_relax(ora.snapshot()), _gpu_state(fresh, s + k))
+        assert not bad, "step %d after a load at step %d: %s" % (s + k, s, "; ".join(bad[:6]))
+    assert ora.tie_count() > 0
