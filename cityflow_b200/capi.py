@@ -88,6 +88,12 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_load_from_file": (i32, [vp, cp]),
         "cfb_set_replay_file": (i32, [vp, cp]),
         "cfb_set_save_replay": (i32, [vp, i32]),
+        "cfb_timed_steps": (i32, [vp, i32, i32, vp, vp]),
+        "cfb_vehicle_steps": (i64, [vp]),
+        "cfb_transfer_bytes": (i32, [vp, vp, vp]),
+        "cfb_debug_launch_form": (i32, [vp, vp]),
+        "cfb_debug_step_grids": (i32, [vp, vp]),
+        "cfb_shard_group_counters": (i32, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         if not hasattr(lib, name):
@@ -217,6 +223,65 @@ class CEngine:
     def tie_count(self) -> int:
         return int(self._check(self.lib.cfb_tie_count(self.h)))
 
+    def launch_form(self) -> tuple:
+        """(graph, pdl, coop, mirror) of the last step (cfb_debug_launch_form)."""
+        a = np.zeros(4, np.int32)
+        self._check(self.lib.cfb_debug_launch_form(self.h, a.ctypes.data))
+        return tuple(int(x) for x in a)
+
+    def step_grids(self) -> dict:
+        """Blocks of the list-driven step kernels (cfb_debug_step_grids); 0 = not launched yet."""
+        a = np.zeros(5, np.int32)
+        self._check(self.lib.cfb_debug_step_grids(self.h, a.ctypes.data))
+        return dict(zip(("k_notify", "k_control", "k_move", "k_leader", "k_step"), (int(x) for x in a)))
+
+    def timed_steps(self, n: int, flush_l2: bool = False):
+        """(device ms, vehicle steps) of n event-bracketed steps (cfb_timed_steps)."""
+        ms, vs = ctypes.c_double(0.0), ctypes.c_int64(0)
+        self._check(self.lib.cfb_timed_steps(self.h, n, int(flush_l2), ctypes.byref(ms), ctypes.byref(vs)))
+        return ms.value, vs.value
+
+    def vehicle_steps(self) -> int:
+        return int(self._check(self.lib.cfb_vehicle_steps(self.h)))
+
+    def enable_kernel_timing(self, on: bool = True):
+        self._check(self.lib.cfb_enable_kernel_timing(self.h, int(on)))
+
+    def kernel_times(self):
+        """(ms per kernel: ingest, notify, control, move, leader; steps timed)"""
+        ms, n = np.zeros(5), ctypes.c_int64(0)
+        self._check(self.lib.cfb_kernel_times(self.h, ms.ctypes.data, ctypes.byref(n)))
+        return ms, n.value
+
+    def transfer_bytes(self):
+        """(host->device, device->host) bytes so far"""
+        h2d, d2h = ctypes.c_int64(0), ctypes.c_int64(0)
+        self._check(self.lib.cfb_transfer_bytes(self.h, ctypes.byref(h2d), ctypes.byref(d2h)))
+        return h2d.value, d2h.value
+
+    def snapshot(self) -> "CArchive":
+        a = self.lib.cfb_snapshot(self.h)
+        if not a:
+            raise RuntimeError(self.lib.cfb_last_error(self.h).decode())
+        return CArchive(self.lib, a)
+
+    def load(self, archive: "CArchive"):
+        self._check(self.lib.cfb_load(self.h, archive.h))
+
+
+class CArchive:
+    """A cfb_snapshot image, freed with the object."""
+
+    def __init__(self, lib, h):
+        self.lib, self.h = lib, h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.cfb_archive_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
 
 class CShardGroup:
     """`world` ranks of one simulation on ONE GPU (loop-back exchanges): checks the seam protocol."""
@@ -247,6 +312,13 @@ class CShardGroup:
         rc = self.lib.cfb_shard_group_lane_counts(self.h, a.ctypes.data, n_lanes, int(waiting))
         assert rc == 0
         return a
+
+    def counters(self):
+        """(vehicle steps, ties) summed over the ranks"""
+        a = np.zeros(2, np.int64)
+        if self.lib.cfb_shard_group_counters(self.h, a.ctypes.data) < 0:
+            raise RuntimeError(self.lib.cfb_shard_group_last_error(self.h).decode())
+        return int(a[0]), int(a[1])
 
     def debug_vehicles(self):
         n = int(self.lib.cfb_shard_group_debug_vehicles(self.h, None, 0))

@@ -476,6 +476,7 @@ struct DeviceSim::Impl {
     cudaGraph_t graphTemplate[2] = {nullptr, nullptr};
     int gridStep = 0;
     cudaGraphExec_t graphExec[2][GRING] = {};
+    int lastForm[4] = {};   // {graph, pdl, coop, mirror} of the last step() (launchForm)
 
     void dropShardGraphs() {
         for (int k = 0; k < 2; ++k) {
@@ -581,6 +582,7 @@ DeviceSim::DeviceSim(const RoadNet &net, const std::vector<VehicleTemplate> &tem
         I.hMirror = hm;
         V.hostMirror = dm;
         if (const char *g = getenv("CITYFLOW_B200_NO_MIRROR")) if (g[0] == '1') V.hostMirror = nullptr;
+        I.lastForm[3] = V.hostMirror != nullptr;
     }
     V.kin = I.kin.p; V.nkin = I.nkin.p; V.gap = I.gap.p; V.leader = I.leader.p; V.ids = I.ids.p; V.nav = I.nav.p;
     V.nbuf = I.nbuf.p; V.count = I.count.p; V.entCnt = I.entCnt.p; V.ent = I.ent.p;
@@ -817,6 +819,13 @@ void DeviceSim::step(const SpawnRec *recs, int n) {
     }
 launched:
     CFB_CUDA(cudaGetLastError());
+    {   // (a graph step that found its ring instance busy and launched plainly still counts as the graph form)
+        const bool coop = !tm && I.useCoop;
+        I.lastForm[0] = !tm && !coop && I.useGraph;
+        I.lastForm[1] = !tm && !coop && I.usePdl;
+        I.lastForm[2] = coop;
+        I.lastForm[3] = V.hostMirror != nullptr;
+    }
     launches_ += (!tm && I.useCoop) ? 1 : 5;
     steps_ += 1;
     I.epochHost += 1;
@@ -1230,6 +1239,15 @@ void DeviceSim::debugCounters(unsigned long long out[8], bool clear) {
 unsigned long long DeviceSim::vehicleSteps() {
     readCtrlImpl(impl_->stream, impl_->hCtrl, impl_->V.ctrl);
     return impl_->hCtrl->vehicleSteps;
+}
+
+void DeviceSim::launchForm(int out[4]) const {
+    for (int k = 0; k < 4; ++k) out[k] = impl_->lastForm[k];
+}
+
+void DeviceSim::stepGrids(int out[5]) const {
+    const Impl &I = *impl_;
+    out[0] = I.gridNotify; out[1] = I.gridControl; out[2] = I.gridMove; out[3] = I.gridLeader; out[4] = I.gridStep;
 }
 
 void DeviceSim::enableKernelTiming(bool on) {

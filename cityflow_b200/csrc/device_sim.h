@@ -227,6 +227,10 @@ public:
     int debugArrays(unsigned *cyc, unsigned *path);   // numPositions() entries each  // CFB_DEBUG_COUNTERS builds only  // device-side sum of the vehicle count after every step
     KernelTimes kernelTimes();
     long long launchesDone() const { return launches_; }
+    // launch form of the last single-GPU step (see cfb_debug_launch_form): {graph, pdl, coop, mirror}
+    void launchForm(int out[4]) const;
+    // blocks of the list-driven step kernels: k_notify, k_control, k_move, k_leader, k_step (0 = not sized yet)
+    void stepGrids(int out[5]) const;
     int numPositions() const;
     int numDrivables() const;
     int device() const;   // CUDA device ordinal the engine lives on

@@ -1631,6 +1631,18 @@ int64_t cfb_finished_vehicle_count(cfb_engine *e) {
     CFB_TRY(e, e->h.cancelAhead(); e->h.drain(); return (int64_t) e->h.finishedCnt;)
 }
 int64_t cfb_gpu_launches(const cfb_engine *e) { return e->h.dev->launchesDone(); }
+int cfb_debug_launch_form(const cfb_engine *e, int32_t out[4]) {
+    int f[4];
+    e->h.dev->launchForm(f);
+    for (int k = 0; k < 4; ++k) out[k] = f[k];
+    return CFB_OK;
+}
+int cfb_debug_step_grids(const cfb_engine *e, int32_t out[5]) {
+    int g[5];
+    e->h.dev->stepGrids(g);
+    for (int k = 0; k < 5; ++k) out[k] = g[k];
+    return CFB_OK;
+}
 int64_t cfb_tie_count(cfb_engine *e) {
     CFB_TRY(e, return (int64_t) e->h.dev->tieCount();)
 }
@@ -2060,32 +2072,41 @@ struct cfb_shard_group {
 };
 
 namespace {
+// A failed copy would leave last step's records in a mailbox and the step would carry on with them: every call is checked,
+// and cfb_shard_group_step reports the failure.
+void loopCheck(cudaError_t err, const char *what) {
+    if (err != cudaSuccess)
+        throw std::runtime_error(std::string("cityflow_b200 CUDA error in the loop-back exchange (") + what + "): " + cudaGetErrorString(err));
+}
 // copies between the ranks' exchange buffers (same device): a[send range for b] -> b[recv range for a]
 void loopExchange(std::vector<cfb::ShardBuffers> &B, bool tails) {
     const int W = (int) B.size();
-    for (int a = 0; a < W; ++a) cudaStreamSynchronize((cudaStream_t) B[a].stream);
+    for (int a = 0; a < W; ++a) loopCheck(cudaStreamSynchronize((cudaStream_t) B[a].stream), "stream synchronize");
     for (int a = 0; a < W; ++a)
         for (int b = 0; b < W; ++b) {
             if (a == b) continue;
             if (tails) {  // owner a -> feeder b: a.tailSend over a's "own" list for peer b; b.tailRecv over b's "feed" list for peer a
                 const size_t n = (size_t) (B[a].inBeg[b + 1] - B[a].inBeg[b]) * B[a].tailBytes;
-                if (n) cudaMemcpy((char *) B[b].tailRecv + (size_t) B[b].outBeg[a] * B[b].tailBytes,
-                                  (char *) B[a].tailSend + (size_t) B[a].inBeg[b] * B[a].tailBytes, n, cudaMemcpyDeviceToDevice);
+                if (n) loopCheck(cudaMemcpy((char *) B[b].tailRecv + (size_t) B[b].outBeg[a] * B[b].tailBytes,
+                                            (char *) B[a].tailSend + (size_t) B[a].inBeg[b] * B[a].tailBytes, n, cudaMemcpyDeviceToDevice),
+                                 "tail records");
             } else {      // feeder a -> owner b
                 const size_t n = (size_t) (B[a].outBeg[b + 1] - B[a].outBeg[b]) * B[a].moverBytes;
-                if (n) cudaMemcpy((char *) B[b].moverRecv + (size_t) B[b].inBeg[a] * B[b].moverBytes,
-                                  (char *) B[a].moverSend + (size_t) B[a].outBeg[b] * B[a].moverBytes, n, cudaMemcpyDeviceToDevice);
+                if (n) loopCheck(cudaMemcpy((char *) B[b].moverRecv + (size_t) B[b].inBeg[a] * B[b].moverBytes,
+                                            (char *) B[a].moverSend + (size_t) B[a].outBeg[b] * B[a].moverBytes, n, cudaMemcpyDeviceToDevice),
+                                 "mover records");
             }
         }
-    cudaDeviceSynchronize();   // D2D cudaMemcpy may return early; the ranks' streams are non-blocking
+    loopCheck(cudaDeviceSynchronize(), "device synchronize");   // D2D cudaMemcpy may return early; the ranks' streams are non-blocking
 }
 void loopAllGatherBlk(std::vector<cfb::ShardBuffers> &B) {
     const int W = (int) B.size();
-    for (int a = 0; a < W; ++a) cudaStreamSynchronize((cudaStream_t) B[a].stream);
+    for (int a = 0; a < W; ++a) loopCheck(cudaStreamSynchronize((cudaStream_t) B[a].stream), "stream synchronize");
     for (int a = 0; a < W; ++a)
         for (int b = 0; b < W; ++b)
-            cudaMemcpy((char *) B[b].blkAll + (size_t) a * B[a].blkBytesPerRank, B[a].blkSend, B[a].blkBytesPerRank, cudaMemcpyDeviceToDevice);
-    cudaDeviceSynchronize();
+            loopCheck(cudaMemcpy((char *) B[b].blkAll + (size_t) a * B[a].blkBytesPerRank, B[a].blkSend, B[a].blkBytesPerRank,
+                                 cudaMemcpyDeviceToDevice), "blocker records");
+    loopCheck(cudaDeviceSynchronize(), "device synchronize");
 }
 }  // namespace
 
@@ -2175,6 +2196,18 @@ int64_t cfb_shard_group_vehicle_count(cfb_shard_group *g) {
     int64_t s = 0;
     for (auto *e : g->ranks) s += e->h.dev->vehicleCount();
     return s;
+}
+
+// sums over the ranks: out = {vehicle steps (cfb_vehicle_steps), same-step entrant ties (cfb_tie_count)}
+int cfb_shard_group_counters(cfb_shard_group *g, int64_t out[2]) {
+    try {
+        out[0] = out[1] = 0;
+        for (auto *e : g->ranks) { out[0] += (int64_t) e->h.dev->vehicleSteps(); out[1] += e->h.dev->tieCount(); }
+        return CFB_OK;
+    } catch (const std::exception &ex) {
+        g->lastError = ex.what();
+        return CFB_ERR_DEVICE;
+    }
 }
 
 // lane counts assembled from the owning ranks; `waiting` selects speed < 0.1 counts

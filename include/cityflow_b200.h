@@ -178,6 +178,8 @@ const char *cfb_shard_group_last_error(const cfb_shard_group *g);
 int64_t cfb_shard_group_vehicle_count(cfb_shard_group *g);
 int cfb_shard_group_lane_counts(cfb_shard_group *g, int32_t *out, int n, int waiting);
 int64_t cfb_shard_group_debug_vehicles(cfb_shard_group *g, void *out, int64_t cap);
+/* sums over the group's ranks: out = {cfb_vehicle_steps, cfb_tie_count} */
+int cfb_shard_group_counters(cfb_shard_group *g, int64_t out[2]);
 
 /* Test support: full dynamic state of every running vehicle, drivable-major in list order.
  * Record = 8 x int32 {flow, index, priority, drivable, leader flow, leader index, blocker flow,
@@ -191,6 +193,16 @@ typedef struct {
     double dis, speed, gap, offset, waiting_time, last_change_time;
 } cfb_lc_vehicle;
 int64_t cfb_debug_lc_vehicles(cfb_engine *e, cfb_lc_vehicle *out, int64_t cap);
+/* Test support: the launch form of the last single-GPU step, out = {graph, pdl, coop, mirror}, each 0 or 1.  graph: the
+ * five step kernels were replayed as one CUDA graph; pdl: they were chained by programmatic dependent launch; coop: the
+ * step ran as the one cooperative kernel k_step; mirror: the vehicle count is read from mapped host memory.  Kernel timing
+ * runs plain launches without PDL.  A default engine on an H100 reports {1, 1, 0, 1}; the CITYFLOW_B200_NO_GRAPH,
+ * _NO_PDL, _COOP and _NO_MIRROR variables (INTEGRATION.md) change it, and so does a driver that cannot capture
+ * programmatic edges (pdl 0).  All zero but mirror before the first step, and for lane-change and sharded steps. */
+int cfb_debug_launch_form(const cfb_engine *e, int32_t out[4]);
+/* Test support: blocks (256 threads each) of the list-driven step kernels, out = {k_notify, k_control, k_move, k_leader,
+ * k_step}: one resident wave each (occupancy x #SM), sized at the first step that launches them, 0 before. */
+int cfb_debug_step_grids(const cfb_engine *e, int32_t out[5]);
 
 /* Measurement support (bench.py): number of our kernels launched so far, per-kernel CUDA-event
  * time accumulators (ms) when enabled, and device-side size figures. */
@@ -205,7 +217,9 @@ int64_t cfb_tie_count(cfb_engine *e);
 /* n steps, each bracketed by CUDA events on the engine's stream (optionally with a 256 MiB L2
  * flush before each bracket); *ms = summed device time, *vehicle_steps = sum of vehicle counts */
 int cfb_timed_steps(cfb_engine *e, int n, int flush_l2, double *ms, int64_t *vehicle_steps);
-/* device-side running sum of get_vehicle_count() after every step since creation / reset */
+/* device-side running sum of get_vehicle_count() after every step since creation.  cfb_reset sets it back to 0.  It
+ * is part of the device state image, so cfb_load / cfb_load_from_file restore the value it had when the snapshot was
+ * taken (the steps run after the snapshot no longer count). */
 int64_t cfb_vehicle_steps(cfb_engine *e);
 /* bytes copied host->device (spawn records) and device->host (control block reads) so far */
 int cfb_transfer_bytes(const cfb_engine *e, int64_t *h2d, int64_t *d2h);

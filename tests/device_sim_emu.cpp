@@ -310,6 +310,8 @@ void DeviceSim::shardConnect(const std::vector<void *> &peerBase) {
 bool DeviceSim::shardIsP2P() const { auto it = g_shardEmu.find(this); return it != g_shardEmu.end() && it->second.connected; }
 bool DeviceSim::shardVehicleCount(int *) { return false; }
 bool DeviceSim::timingOn() const { return false; }
+void DeviceSim::launchForm(int out[4]) const { for (int k = 0; k < 4; ++k) out[k] = 0; }   // no graph, no PDL, no grid, no mirror
+void DeviceSim::stepGrids(int out[5]) const { for (int k = 0; k < 4; ++k) out[k] = G; out[4] = 0; }
 void DeviceSim::shardTimeMark(int) {}
 void DeviceSim::shardTimeCollect() {}
 void DeviceSim::shardPhaseTimes(double *ms, long long *steps) { for (int k = 0; k < SHARD_PHASES; ++k) ms[k] = 0; if (steps) *steps = 0; }

@@ -329,6 +329,21 @@ def write(shape: str, directory: str, seed: int = 1, lane_change: bool = False) 
                                    name="%s%d%s" % (shape, seed, "_lc" if lane_change else ""))
 
 
+def write_spawn_burst(directory: str, n_flows: int = 2200) -> str:
+    """A 4x4 grid with `n_flows` single-vehicle flows that all start at t = 0, so that the first step hands the device more
+    spawn records than k_ingest stages in shared memory (SPAWN_SMEM = 2048)."""
+    from cityflow_b200 import scenario
+    net = scenario.grid_roadnet(4, 4)
+    base = scenario.random_walk_flows(net, frac=1.0, interval=5.0, seed=4)
+    flows = []
+    for k in range(n_flows):
+        f = dict(base[k % len(base)])
+        f["vehicle"] = dict(f["vehicle"])
+        f["interval"], f["startTime"], f["endTime"] = 1.0, 0, 0
+        flows.append(f)
+    return scenario.write_scenario(directory, net, flows, seed=5, name="burst")
+
+
 def loader_tables(cfg: str) -> dict:
     """The static tables of the product's loader (tests/loader_probe.cpp, built into oracle/_build like
     tests/test_cpu.py's _dump_static): lane_out, link_end, link_cross_count, ..."""
