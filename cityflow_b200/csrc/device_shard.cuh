@@ -1,4 +1,5 @@
-// device_shard.cuh -- the seam protocol of a sharded run over PEER MEMORY (NVLink / NVSwitch).
+// device_shard.cuh -- what crosses a seam of a sharded run (partition.h, shard.h): the seam records, and the protocol
+// that moves them over PEER MEMORY (NVLink / NVSwitch) or, staged, through a ShardTransport.
 // Part of device_sim.cu.  The reference has no counterpart (its threads share one address space).
 //
 // Every rank owns one "arena" (one cudaMalloc, exported with cudaIpc and mapped by every peer):
@@ -132,64 +133,106 @@ __device__ __forceinline__ void shardPdlEnter() {
 #endif
 }
 
+// ---- the seam records, one definition each: the peer-memory bodies below and the staged kernels (k_pack_* / k_unpack_*)
+// differ only in where a record is stored and where it is read from ----
+
+// Owner side: the tail record of boundary lane L (Drivable::getLastVehicle) with the state of that vehicle.
+__device__ __forceinline__ TailMsg tailMsgOf(const View &V, int L) {
+    TailMsg m;
+    m.tail = V.tail[L];
+    m.count = V.count[L];
+    m.inserted = V.inserted[L];
+    m.pad0 = m.pad1 = 0;
+    m.kin = make_double2(0, 0);
+    m.ids = m.nav = make_int4(0, 0, 0, 0);
+    if (m.tail.pos >= 0) {
+        m.kin = V.kin[m.tail.pos];
+        m.ids = V.ids[m.tail.pos];
+        m.nav = V.nav[m.tail.pos];
+    }
+    return m;
+}
+// Feeder side: refresh boundary lane L from its owner's tail record.
+__device__ __forceinline__ void applyTailMsg(const View &V, int L, const TailMsg m) {   // (a copy: every load before the stores)
+    V.tail[L] = m.tail;
+    V.count[L] = m.count;
+    V.inserted[L] = (unsigned char) m.inserted;
+    if (m.tail.pos >= 0) {  // ghost copy of the one vehicle this rank may look at
+        V.kin[m.tail.pos] = m.kin;
+        V.ids[m.tail.pos] = m.ids;
+        V.nav[m.tail.pos] = m.nav;
+    }
+}
+// Feeder side, one warp per lane: this step's entrants of boundary lane L into `out`; they leave this rank.
+__device__ __forceinline__ void fillMoverMsg(const View &V, int L, MoverMsg *out, int lane) {
+    const int n = min(V.entCnt[L], ENT_CAP);
+    if (lane == 0) { out->n = n; out->pad0 = out->pad1 = out->pad2 = 0; }
+    if (lane < n) {
+        const int m = V.ent[L * ENT_CAP + lane];
+        MoverRec r;
+        r.kin = V.mkin[m];
+        r.ids = V.mids[m];
+        r.nav = V.mnav[m];
+        out->rec[lane] = r;
+    }
+    __syncwarp();
+    if (lane == 0) V.entCnt[L] = 0;
+}
+// Owner side, one warp per lane: stage the entrants of boundary lane L like local movers.
+__device__ __forceinline__ void stageMoverMsg(const View &V, int L, const MoverMsg *in, int lane) {
+    const int n = in->n;
+    if (n == 0) return;
+    int base = 0;
+    if (lane == 0) base = atomicAdd(&V.ctrl->moverCount, n);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (lane < n) {
+        const int m = base + lane;
+        if (m < V.moverCap) {
+            const MoverRec r = in->rec[lane];
+            V.mkin[m] = r.kin;
+            V.mids[m] = r.ids;
+            V.mnav[m] = r.nav;
+            V.ent[L * ENT_CAP + lane] = m;
+        } else {
+            atomicOr(&V.ctrl->error, ERR_MOVER_OVERFLOW);
+        }
+    }
+    if (lane == 0) {
+        V.entCnt[L] = n;
+        if (V.count[L] == 0) V.extraList[atomicAdd(&V.ctrl->nExtra, 1)] = L;
+    }
+}
+// One blocker change of another rank: u = (slot, blocker slot), blocker -2 = the vehicle left the network at `step`.
+__device__ __forceinline__ void applyBlkChange(const View &V, int2 u, int step) {
+    if (u.y == -2) {
+        V.blk[u.x] = -1;
+        V.delStep[u.x] = step;
+    } else {
+        V.blk[u.x] = u.y;
+    }
+}
+
 // After k_control: one warp per boundary lane this rank feeds; the record goes straight into the owner's arena.
 __device__ __forceinline__ void sendMoversBody(const View &V, const ShardP2P &S) {
     const int E = V.ctrl->epoch + 1, par = E & 1;
-    const int lane = threadIdx.x & 31;
     const int nW = (gridDim.x * blockDim.x) >> 5;
     for (int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < V.nBoundOut; j += nW) {
-        const int L = V.boundOut[j];
         const ShardPeer &P = S.peers[S.outPeer[j]];
-        MoverMsg *out = P.moverIn + (size_t) par * P.nIn + S.outDst[j];
-        const int n = min(V.entCnt[L], ENT_CAP);
-        if (lane == 0) { out->n = n; out->pad0 = out->pad1 = out->pad2 = 0; }
-        if (lane < n) {
-            const int m = V.ent[L * ENT_CAP + lane];
-            MoverRec r;
-            r.kin = V.mkin[m];
-            r.ids = V.mids[m];
-            r.nav = V.mnav[m];
-            out->rec[lane] = r;
-        }
-        __syncwarp();
-        if (lane == 0) V.entCnt[L] = 0;
+        fillMoverMsg(V, V.boundOut[j], P.moverIn + (size_t) par * P.nIn + S.outDst[j], threadIdx.x & 31);
     }
     if (shardLastBlock(S.ticket) && threadIdx.x == 0)   // (the thread that issued the system fence)
         for (int k = 0; k < S.nNbr; ++k) *(volatile int *) (S.peers[S.nbr[k]].flags + 0 * S.world + S.me) = E;
 }
 __global__ void __launch_bounds__(128) k_send_movers(View V, ShardP2P S) { shardPdlEnter(); sendMoversBody(V, S); }
 
-// Before k_move: wait for the feeders, then stage their entrants like local movers (cf. k_unpack_movers).
+// Before k_move: wait for the feeders, then stage their entrants like local movers.
 __device__ __forceinline__ void recvMoversBody(const View &V, const ShardP2P &S) {
     const int E = V.ctrl->epoch + 1, par = E & 1;
     shardWait(V, S, 0, E, false);
-    const int lane = threadIdx.x & 31;
     const int nW = (gridDim.x * blockDim.x) >> 5;
     const MoverMsg *in = S.moverIn + (size_t) par * V.nBoundIn;
-    for (int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < V.nBoundIn; j += nW) {
-        const int L = V.boundIn[j];
-        const int n = in[j].n;
-        if (n == 0) continue;
-        int base = 0;
-        if (lane == 0) base = atomicAdd(&V.ctrl->moverCount, n);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (lane < n) {
-            const int m = base + lane;
-            if (m < V.moverCap) {
-                const MoverRec r = in[j].rec[lane];
-                V.mkin[m] = r.kin;
-                V.mids[m] = r.ids;
-                V.mnav[m] = r.nav;
-                V.ent[L * ENT_CAP + lane] = m;
-            } else {
-                atomicOr(&V.ctrl->error, ERR_MOVER_OVERFLOW);
-            }
-        }
-        if (lane == 0) {
-            V.entCnt[L] = n;
-            if (V.count[L] == 0) V.extraList[atomicAdd(&V.ctrl->nExtra, 1)] = L;
-        }
-    }
+    for (int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < V.nBoundIn; j += nW)
+        stageMoverMsg(V, V.boundIn[j], in + j, threadIdx.x & 31);
 }
 __global__ void __launch_bounds__(128) k_recv_movers(View V, ShardP2P S) { shardPdlEnter(); recvMoversBody(V, S); }
 // Both halves in one launch (the default): this rank's sends do not depend on what it receives, so the kernel first
@@ -202,21 +245,8 @@ __device__ __forceinline__ void sendTailsBody(const View &V, const ShardP2P &S) 
     const int E = V.ctrl->epoch + 1, par = E & 1;
     const int gtid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
     for (int j = gtid; j < V.nBoundIn; j += stride) {
-        const int L = V.boundIn[j];
-        TailMsg m;
-        m.tail = V.tail[L];
-        m.count = V.count[L];
-        m.inserted = V.inserted[L];
-        m.pad0 = m.pad1 = 0;
-        m.kin = make_double2(0, 0);
-        m.ids = m.nav = make_int4(0, 0, 0, 0);
-        if (m.tail.pos >= 0) {
-            m.kin = V.kin[m.tail.pos];
-            m.ids = V.ids[m.tail.pos];
-            m.nav = V.nav[m.tail.pos];
-        }
         const ShardPeer &P = S.peers[S.inPeer[j]];
-        P.tailIn[(size_t) par * P.nOut + S.inDst[j]] = m;
+        P.tailIn[(size_t) par * P.nOut + S.inDst[j]] = tailMsgOf(V, V.boundIn[j]);
     }
     const int nUpd = V.ctrl->nBlkUpd;
     if (nUpd > BLK_IN_CAP) atomicOr(&V.ctrl->error, ERR_MOVER_OVERFLOW);
@@ -253,36 +283,49 @@ __device__ __forceinline__ void recvTailsBody(const View &V, const ShardP2P &S) 
     shardWait(V, S, 1, E, false);
     const int gtid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
     const TailMsg *in = S.tailIn + (size_t) par * V.nBoundOut;
-    for (int j = gtid; j < V.nBoundOut; j += stride) {
-        const int L = V.boundOut[j];
-        const TailMsg m = in[j];
-        V.tail[L] = m.tail;
-        V.count[L] = m.count;
-        V.inserted[L] = (unsigned char) m.inserted;
-        if (m.tail.pos >= 0) {  // ghost copy of the one vehicle this rank may look at
-            V.kin[m.tail.pos] = m.kin;
-            V.ids[m.tail.pos] = m.ids;
-            V.nav[m.tail.pos] = m.nav;
-        }
-    }
+    for (int j = gtid; j < V.nBoundOut; j += stride) applyTailMsg(V, V.boundOut[j], in[j]);
     const size_t blkStride = (size_t) S.world * (1 + BLK_IN_CAP);
     const int step = V.ctrl->step;
     for (int k = 0; k < S.nNbr; ++k) {
         const int2 *src = S.blkIn + (size_t) par * blkStride + (size_t) S.nbr[k] * (1 + BLK_IN_CAP);
         const int n = src[0].x;
-        for (int i = gtid; i < n; i += stride) {
-            const int2 u = src[1 + i];
-            if (u.y == -2) {
-                V.blk[u.x] = -1;
-                V.delStep[u.x] = step;
-            } else {
-                V.blk[u.x] = u.y;
-            }
-        }
+        for (int i = gtid; i < n; i += stride) applyBlkChange(V, src[1 + i], step);
     }
 }
 __global__ void __launch_bounds__(128) k_recv_tails(View V, ShardP2P S) { shardPdlEnter(); recvTailsBody(V, S); }
 __global__ void __launch_bounds__(128) k_xchg_tails(View V, ShardP2P S) { shardPdlEnter(); sendTailsBody(V, S); recvTailsBody(V, S); }
+
+// ---- the staged form: the same records through the engine's send / receive buffers, moved between the ranks by a
+// ShardTransport (CITYFLOW_B200_SHARD_TRANSPORT=nccl) ----
+__global__ void k_pack_tails(View V, TailMsg *out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < V.nBoundIn) out[j] = tailMsgOf(V, V.boundIn[j]);
+}
+__global__ void k_unpack_tails(View V, const TailMsg *in) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < V.nBoundOut) applyTailMsg(V, V.boundOut[j], in[j]);
+}
+__global__ void k_pack_movers(View V, MoverMsg *out) {  // one warp per boundary lane this rank feeds
+    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (j < V.nBoundOut) fillMoverMsg(V, V.boundOut[j], out + j, threadIdx.x & 31);
+}
+__global__ void k_unpack_movers(View V, const MoverMsg *in) {  // one warp per boundary lane this rank owns
+    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (j < V.nBoundIn) stageMoverMsg(V, V.boundIn[j], in + j, threadIdx.x & 31);
+}
+// blocker changes: [0] = {count,0} header, filled right before the all-gather
+__global__ void k_seal_blk(View V) {
+    V.blkUpd[0] = make_int2(min(V.ctrl->nBlkUpd, V.blkUpdCap), 0);
+    V.ctrl->nBlkUpd = 0;
+}
+// every other rank's list, one rank per blockIdx.y
+__global__ void k_apply_blk(View V, const int2 *all, int me, int stridePerRank) {
+    const int r = blockIdx.y;
+    if (r == me) return;
+    const int2 *src = all + (size_t) r * stridePerRank;
+    const int n = src[0].x, step = V.ctrl->step;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) applyBlkChange(V, src[1 + i], step);
+}
 
 // Host query support: every rank's finished-vehicle marks through the last completed step have landed here.
 __global__ void k_wait_fin(View V, ShardP2P S) { shardWait(V, S, 2, V.ctrl->epoch, true); }

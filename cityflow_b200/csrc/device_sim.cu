@@ -108,93 +108,10 @@ __global__ void __launch_bounds__(256, 4) k_step(View V) {
 }
 
 // ------------------------------------------------------------------------------------------
-// Sharded mode: what crosses a seam (partition.h).  Fixed-size messages, one entry per boundary lane
-// (TailMsg / MoverMsg in device_shard.cuh, with the peer-memory transport).  The k_pack / k_unpack / k_seal /
-// k_apply kernels below are the staging form used with the NCCL transport (CITYFLOW_B200_SHARD_TRANSPORT=nccl).
+// Sharded mode: the seam records and both of their transports (device_shard.cuh).
 }  // namespace cfb
 #include "device_shard.cuh"
 namespace cfb {
-
-__global__ void k_pack_tails(View V, TailMsg *out) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= V.nBoundIn) return;
-    const int L = V.boundIn[j];
-    TailMsg m;
-    m.tail = V.tail[L];
-    m.count = V.count[L];
-    m.inserted = V.inserted[L];
-    m.pad0 = m.pad1 = 0;
-    m.kin = make_double2(0, 0);
-    m.ids = m.nav = make_int4(0, 0, 0, 0);
-    if (m.tail.pos >= 0) {
-        m.kin = V.kin[m.tail.pos];
-        m.ids = V.ids[m.tail.pos];
-        m.nav = V.nav[m.tail.pos];
-    }
-    out[j] = m;
-}
-
-__global__ void k_unpack_tails(View V, const TailMsg *in) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= V.nBoundOut) return;
-    const int L = V.boundOut[j];
-    const TailMsg m = in[j];
-    V.tail[L] = m.tail;
-    V.count[L] = m.count;
-    V.inserted[L] = (unsigned char) m.inserted;
-    if (m.tail.pos >= 0) {  // ghost copy of the one vehicle this rank may look at
-        V.kin[m.tail.pos] = m.kin;
-        V.ids[m.tail.pos] = m.ids;
-        V.nav[m.tail.pos] = m.nav;
-    }
-}
-
-__global__ void k_pack_movers(View V, MoverMsg *out) {  // one warp per boundary lane this rank feeds
-    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (j >= V.nBoundOut) return;
-    const int L = V.boundOut[j];
-    const int n = min(V.entCnt[L], ENT_CAP);
-    if (lane == 0) { out[j].n = n; out[j].pad0 = out[j].pad1 = out[j].pad2 = 0; }
-    if (lane < n) {
-        const int m = V.ent[L * ENT_CAP + lane];
-        MoverRec r;
-        r.kin = V.mkin[m];
-        r.ids = V.mids[m];
-        r.nav = V.mnav[m];
-        out[j].rec[lane] = r;
-    }
-    __syncwarp();
-    if (lane == 0) V.entCnt[L] = 0;
-}
-
-__global__ void k_unpack_movers(View V, const MoverMsg *in) {  // one warp per boundary lane this rank owns
-    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (j >= V.nBoundIn) return;
-    const int L = V.boundIn[j];
-    const int n = in[j].n;
-    if (n == 0) return;
-    int base = 0;
-    if (lane == 0) base = atomicAdd(&V.ctrl->moverCount, n);
-    base = __shfl_sync(0xffffffffu, base, 0);
-    if (lane < n) {
-        const int m = base + lane;
-        if (m < V.moverCap) {
-            const MoverRec r = in[j].rec[lane];
-            V.mkin[m] = r.kin;
-            V.mids[m] = r.ids;
-            V.mnav[m] = r.nav;
-            V.ent[L * ENT_CAP + lane] = m;
-        } else {
-            atomicOr(&V.ctrl->error, ERR_MOVER_OVERFLOW);
-        }
-    }
-    if (lane == 0) {
-        V.entCnt[L] = n;
-        if (V.count[L] == 0) V.extraList[atomicAdd(&V.ctrl->nExtra, 1)] = L;
-    }
-}
 
 __global__ void k_mask_counts(View V, int *out) {  // out[0] = vehicles this rank accounts for, out[1+l] = owned lane counts
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -204,27 +121,6 @@ __global__ void k_mask_counts(View V, int *out) {  // out[0] = vehicles this ran
 __global__ void k_mask_waiting(View V, const int *waiting, int *out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < V.nLanes) out[i] = (!V.owned || V.owned[i] == 1) ? waiting[i] : 0;
-}
-
-// blocker changes: [0] = {count,0} header, filled right before the all-gather
-__global__ void k_seal_blk(View V) {
-    V.blkUpd[0] = make_int2(min(V.ctrl->nBlkUpd, V.blkUpdCap), 0);
-    V.ctrl->nBlkUpd = 0;
-}
-__global__ void k_apply_blk(View V, const int2 *all, int world, int me, int stridePerRank) {
-    const int r = blockIdx.y;
-    if (r == me) return;
-    const int2 *src = all + (size_t) r * stridePerRank;
-    const int n = src[0].x;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const int2 u = src[1 + i];
-        if (u.y == -2) {
-            V.blk[u.x] = -1;
-            V.delStep[u.x] = V.ctrl->step;
-        } else {
-            V.blk[u.x] = u.y;
-        }
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -354,6 +250,37 @@ static void launchPdl(void (*k)(A...), int grid, int block, cudaStream_t s, bool
     CFB_CUDA(cudaLaunchKernelEx(&cfg, k, args...));
 }
 
+// A step replayed as ONE CUDA graph per list parity.  Re-launching an executable graph whose previous launch has not
+// finished makes the driver wait on the host (observed: ~1 ms per step), so each parity has a small ring of instances of
+// the same graph: the host may run 2 * GRING steps ahead of the device before a step falls back to plain launches.
+struct GraphRing {
+    static constexpr int GRING = 4;
+    cudaGraph_t tmpl[2] = {nullptr, nullptr};   // the captured step, per parity
+    cudaGraphExec_t exec[2][GRING] = {};
+    cudaEvent_t done[2][GRING] = {};
+    static int slot(long long steps) { return (int) ((steps >> 1) % GRING); }   // the instance of the step after `steps`
+    bool instantiate(int par, int r) { return cudaGraphInstantiate(&exec[par][r], tmpl[par], 0) == cudaSuccess; }
+    // the instance's last launch has not finished
+    bool busy(int par, int r) const { return done[par][r] && cudaEventQuery(done[par][r]) != cudaSuccess; }
+    void launch(int par, int r, cudaStream_t s) {
+        if (!done[par][r]) CFB_CUDA(cudaEventCreateWithFlags(&done[par][r], cudaEventDisableTiming));
+        CFB_CUDA(cudaGraphLaunch(exec[par][r], s));
+        CFB_CUDA(cudaEventRecord(done[par][r], s));
+    }
+    void drop(cudaStream_t s) {
+        for (int k = 0; k < 2; ++k) {
+            for (int r = 0; r < GRING; ++r)
+                if (exec[k][r]) { cudaStreamSynchronize(s); cudaGraphExecDestroy(exec[k][r]); exec[k][r] = nullptr; }
+            if (tmpl[k]) { cudaGraphDestroy(tmpl[k]); tmpl[k] = nullptr; }
+        }
+    }
+    void release(cudaStream_t s) {
+        drop(s);
+        for (auto &row : done)
+            for (cudaEvent_t &e : row) if (e) cudaEventDestroy(e);
+    }
+};
+
 struct DeviceSim::Impl {
     DeviceSimOptions opt;
     View V{};
@@ -380,14 +307,8 @@ struct DeviceSim::Impl {
     std::vector<int> outBeg, inBeg;
     std::vector<unsigned char> ownedHost;
     int shardRank = 0, shardWorld = 1;
-    // A step is replayed as ONE graph per list parity.  Re-launching an executable graph whose previous launch has not
-    // finished makes the driver wait on the host, so each parity has a small ring of instances of the same graph: the
-    // host may run 2 * GRING steps ahead of the device before a step falls back to plain launches.
-    static constexpr int GRING = 4;
-    cudaGraph_t shardTemplate[2] = {nullptr, nullptr};
-    cudaGraphExec_t shardGraph[2][GRING] = {};
-    cudaEvent_t shardGraphDone[2][GRING] = {};
-    bool shardGraphOk = true;    // whole sharded step (kernels + NCCL groups) replayed as one graph per parity
+    GraphRing shardGraphs;       // the whole sharded step (kernels + NCCL groups)
+    bool shardGraphOk = true;
     DevBuf<int> shardScratch;
     DevBuf<unsigned char> finGather;
     // peer-memory transport (device_shard.cuh)
@@ -471,26 +392,164 @@ struct DeviceSim::Impl {
     int gridNotify = 0, gridMove = 0, gridLeader = 0, gridControl = 0;
     bool mirrorStale = false;   // something other than a step changed active / error (reset, restore, a setter): read the device
     bool usePdl = true;   // CITYFLOW_B200_NO_PDL=1: plain stream order between the step kernels
-    bool useGraph = true, graphDirty = false, useCoop = false;   // cooperative k_step measured slower (DESIGN.md §4)
-    cudaEvent_t graphDone[2][GRING] = {};
-    cudaGraph_t graphTemplate[2] = {nullptr, nullptr};
+    bool useGraph = true, useCoop = false;   // cooperative k_step measured slower (DESIGN.md §4)
+    GraphRing graphs;        // the five kernels of a single-GPU step
     int gridStep = 0;
-    cudaGraphExec_t graphExec[2][GRING] = {};
     int lastForm[4] = {};   // {graph, pdl, coop, mirror} of the last step() (launchForm)
 
-    void dropShardGraphs() {
-        for (int k = 0; k < 2; ++k) {
-            for (int r = 0; r < GRING; ++r)
-                if (shardGraph[k][r]) { cudaStreamSynchronize(stream); cudaGraphExecDestroy(shardGraph[k][r]); shardGraph[k][r] = nullptr; }
-            if (shardTemplate[k]) { cudaGraphDestroy(shardTemplate[k]); shardTemplate[k] = nullptr; }
+    // The graphs bake in the View's pointers: every change of a device buffer or table drops them (rebuilt on use).
+    void invalidateGraphs() {
+        graphs.drop(stream);
+        shardGraphs.drop(stream);
+    }
+    // Grids of the list-driven step kernels: one resident wave each (occupancy x #SM blocks, grid-stride loops inside).
+    void ensureGrids() {
+        if (gridNotify) return;
+        int b = 0;
+        CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_notify, 256, 0)); gridNotify = std::max(b, 1) * numSMs;
+        CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_move, 256, 0)); gridMove = std::max(b, 1) * numSMs;
+        CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_leader, 256, 0)); gridLeader = std::max(b, 1) * numSMs;
+        CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_control, 256, 0)); gridControl = std::max(b, 1) * numSMs;
+    }
+    // The five step kernels, each with its one launch description.  k_ingest covers its lane / roadLink lists (a rank of a
+    // sharded run: only those it ingests into) and follows a copy, never a kernel, so it is never chained by PDL; `pdl`
+    // chains the others behind the kernel before them (see pdlEnter()).
+    enum StepKernel { INGEST, NOTIFY, CONTROL, MOVE, LEADER };
+    void launchStep(StepKernel k, bool pdl) {
+        static void (*const kernel[5])(View) = {k_ingest, k_notify, k_control, k_move, k_leader};
+        ensureGrids();
+        const int TPB = 256;
+        const int ingest = (V.ingLanes ? std::max(std::max(V.nIngLanes, V.nIngRL), V.nIngLinks * V.maskWords / 4)
+                                       : std::max(V.nLanes, V.nRL)) + TPB - 1;
+        const int grid[5] = {std::max(ingest / TPB, 1), gridNotify, gridControl, gridMove, gridLeader};
+        launchPdl(kernel[k], grid[k], TPB, stream, pdl && k != INGEST, V);
+    }
+    bool pdl() const { return usePdl && !timing; }   // (events between the kernels would serialise them anyway)
+
+    // ---- the sharded step (DeviceSim::shardStep / shardSegment) ----
+    void shardTimeMark(int k) {
+        if (!shardEv[k]) CFB_CUDA(cudaEventCreate(&shardEv[k]));
+        CFB_CUDA(cudaEventRecord(shardEv[k], stream));
+    }
+    void shardTimeCollect() {   // after mark SHARD_PHASES: accumulates the phase durations
+        CFB_CUDA(cudaEventSynchronize(shardEv[SHARD_PHASES]));
+        for (int k = 0; k < SHARD_PHASES; ++k) {
+            float ms = 0;
+            cudaEventElapsedTime(&ms, shardEv[k], shardEv[k + 1]);
+            shardMs[k] += ms;
+        }
+        shardTimedSteps += 1;
+    }
+    // The seam kernels of the peer-memory form: a warp per boundary lane for the movers, 16 blocks for the tails.
+    static int moverGrid(int lanes) { return std::max(1, std::min(64, (lanes * 32 + 127) / 128)); }
+    static constexpr int TAIL_GRID = 16;
+    void launchSeam(void (*k)(View, ShardP2P), int grid) { launchPdl(k, grid, 128, stream, pdl(), V, S); }
+    // Segment k of the step, the work between two seam exchanges (see DeviceSim::shardSegment), over peer memory when
+    // connected, else through the staging buffers.  `marks`: record the phase events of kernel timing (peer memory).
+    void shardSegment(int k, bool marks, long long &launches) {
+        auto mark = [&](int e) { if (marks) shardTimeMark(e); };
+        if (k == 0) {
+            mark(0);
+            launchStep(INGEST, false);
+            mark(1);
+            launchStep(NOTIFY, pdl());
+            launchStep(CONTROL, pdl());
+            mark(2);
+            if (p2p) launchSeam(k_send_movers, moverGrid(V.nBoundOut));   // X1
+            else if (V.nBoundOut) k_pack_movers<<<(V.nBoundOut * 32 + 127) / 128, 128, 0, stream>>>(V, moverSend.p);
+            launches += 4;
+        } else if (k == 1) {
+            mark(3);
+            if (p2p) launchSeam(k_recv_movers, moverGrid(V.nBoundIn));
+            else if (V.nBoundIn) k_unpack_movers<<<(V.nBoundIn * 32 + 127) / 128, 128, 0, stream>>>(V, moverRecv.p);
+            mark(4);
+            launchStep(MOVE, pdl());
+            mark(5);
+            if (p2p) {
+                launchSeam(k_send_tails, TAIL_GRID);   // X2
+            } else {
+                if (V.nBoundIn) k_pack_tails<<<(V.nBoundIn + 127) / 128, 128, 0, stream>>>(V, tailSend.p);
+                k_seal_blk<<<1, 1, 0, stream>>>(V);
+            }
+            launches += p2p ? 3 : 4;
+        } else {
+            mark(6);
+            if (p2p) {
+                launchSeam(k_recv_tails, TAIL_GRID);
+            } else {
+                if (V.nBoundOut) k_unpack_tails<<<(V.nBoundOut + 127) / 128, 128, 0, stream>>>(V, tailRecv.p);
+                k_apply_blk<<<dim3(32, shardWorld), 256, 0, stream>>>(V, blkAll.p, shardRank, 1 + V.blkUpdCap);
+            }
+            mark(7);
+            launchStep(LEADER, pdl());
+            mark(8);
+            if (marks) shardTimeCollect();
+            launches += p2p ? 2 : 3;
         }
     }
-    void dropGraphs() {
-        for (int k = 0; k < 2; ++k) {
-            for (int r = 0; r < GRING; ++r)
-                if (graphExec[k][r]) { cudaStreamSynchronize(stream); cudaGraphExecDestroy(graphExec[k][r]); graphExec[k][r] = nullptr; }
-            if (graphTemplate[k]) { cudaGraphDestroy(graphTemplate[k]); graphTemplate[k] = nullptr; }
+    // The kernels of one sharded step.  Peer memory: by default 7 kernels (ingest, notify, control, exchange movers, move,
+    // exchange tails, leader), nothing but kernels on the stream; split into separate send / receive kernels with
+    // CITYFLOW_B200_SHARD_SPLIT=1 or kernel timing, which records the eight phases.  Staged: the three segments with
+    // t's two exchanges in between.
+    void shardKernels(ShardTransport *t, long long &launches) {
+        if (p2p && !shardSplit && !timing) {
+            launchStep(INGEST, false);
+            launchStep(NOTIFY, pdl());
+            launchStep(CONTROL, pdl());
+            launchSeam(k_xchg_movers, moverGrid(std::max(V.nBoundOut, V.nBoundIn)));   // X1
+            launchStep(MOVE, pdl());
+            launchSeam(k_xchg_tails, TAIL_GRID);   // X2
+            launchStep(LEADER, pdl());
+            launches += 7;
+        } else if (p2p) {
+            for (int k = 0; k < 3; ++k) shardSegment(k, timing, launches);
+        } else {
+            shardSegment(0, false, launches);
+            t->exchange(stream, moverSend.p, outBeg, moverRecv.p, inBeg, sizeof(MoverMsg));   // X1
+            shardSegment(1, false, launches);
+            t->exchangeAndGather(stream, tailSend.p, inBeg, tailRecv.p, outBeg, sizeof(TailMsg),
+                                 blkUpd.p, blkAll.p, (size_t) (1 + V.blkUpdCap) * sizeof(int2));   // X2
+            shardSegment(2, false, launches);
         }
+    }
+    // The sharded step of `steps` is captured into a CUDA graph per list parity and replayed: one launch call per step
+    // instead of ~17.  The first steps run uncaptured so that NCCL can set up its connections; any capture failure
+    // switches the engine back to plain launches for good.  Returns 0 plain, 1 replayed (nothing left to enqueue),
+    // 2 capturing (enqueue the kernels, then shardGraphEnd).
+    int shardGraphBegin(long long steps) {
+        const int par = V.par, r = GraphRing::slot(steps);
+        if (!shardGraphOk || steps < 8 || timing) return 0;
+        GraphRing &G = shardGraphs;
+        if (G.exec[par][r] || G.tmpl[par]) {
+            if (!G.exec[par][r] && !G.instantiate(par, r)) { cudaGetLastError(); G.exec[par][r] = nullptr; return 0; }
+            else if (G.busy(par, r)) { cudaGetLastError(); return 0; }   // this instance is still running: just enqueue
+            G.launch(par, r, stream);
+            return 1;
+        }
+        if (cudaStreamBeginCapture(stream, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
+            cudaGetLastError();
+            shardGraphOk = false;
+            return 0;
+        }
+        return 2;
+    }
+    bool shardGraphEnd(int state, long long steps) {   // false: capture failed, nothing ran -> repeat the step plainly
+        if (state != 2) return true;
+        const int par = V.par, r = GraphRing::slot(steps);
+        GraphRing &G = shardGraphs;
+        cudaGraph_t g = nullptr;
+        cudaError_t e = cudaStreamEndCapture(stream, &g);
+        if (e == cudaSuccess && g) e = cudaGraphInstantiate(&G.exec[par][r], g, 0);
+        if (e != cudaSuccess || !G.exec[par][r]) {
+            if (g) cudaGraphDestroy(g);
+            cudaGetLastError();
+            G.exec[par][r] = nullptr;
+            shardGraphOk = false;
+            return false;
+        }
+        G.tmpl[par] = g;
+        G.launch(par, r, stream);
+        return true;
     }
     void ensureHostInts(size_t n) {
         if (n <= hIntsCap) return;
@@ -606,13 +665,8 @@ DeviceSim::~DeviceSim() {
     }
     for (auto &ev : I.ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : I.stepEv) cudaEventDestroy(ev);
-    I.dropGraphs();
-    I.dropShardGraphs();
-    for (int k = 0; k < 2; ++k)
-        for (int r = 0; r < Impl::GRING; ++r) {
-            if (I.graphDone[k][r]) cudaEventDestroy(I.graphDone[k][r]);
-            if (I.shardGraphDone[k][r]) cudaEventDestroy(I.shardGraphDone[k][r]);
-        }
+    I.graphs.release(I.stream);
+    I.shardGraphs.release(I.stream);
     if (I.hCtrl) cudaFreeHost(I.hCtrl);
     if (I.hMirror) cudaFreeHost((void *) I.hMirror);
     if (I.hInts) cudaFreeHost(I.hInts);
@@ -632,8 +686,7 @@ void DeviceSim::uploadTemplates(const std::vector<VehicleTemplate> &templates) {
     CFB_CUDA(cudaStreamSynchronize(I.stream));
     I.tmpl.upload(t);
     I.V.tmpl = I.tmpl.p;
-    I.graphDirty = true;
-    I.dropShardGraphs();
+    I.invalidateGraphs();
     legacySync();
 }
 
@@ -645,8 +698,7 @@ void DeviceSim::uploadPlans(const Routing &routing) {
     I.planData.upload(T.planData);
     I.V.planBeg = I.planBeg.p;
     I.V.planData = I.planData.p;
-    I.graphDirty = true;
-    I.dropShardGraphs();
+    I.invalidateGraphs();
     legacySync();
 }
 
@@ -690,8 +742,7 @@ void DeviceSim::ensureSlotCapacity(int slots) {
     legacySync();   // ... and the copies before the old buffers are freed / the new ones are used
     I.slotCap = cap;
     I.V.pos = I.pos.p; I.V.waitNext = I.waitNext.p; I.V.slotInfo = I.slotInfo.p; I.V.slotCust = I.slotCust.p; I.V.blk = I.blk.p; I.V.delStep = I.delStep.p;
-    I.graphDirty = true;
-    I.dropShardGraphs();
+    I.invalidateGraphs();
 }
 
 void DeviceSim::reset() {
@@ -722,8 +773,7 @@ void DeviceSim::stageStep(const SpawnRec *recs, int n) {
         CFB_CUDA(cudaStreamSynchronize(s));
         I.spawnCap = std::max(1024, (n + 1) * 2);
         I.spawn.alloc(I.spawnCap);
-        I.graphDirty = true;
-        I.dropShardGraphs();
+        I.invalidateGraphs();
     }
     V.spawn = I.spawn.p + 1;
     const int r = I.ringIdx;
@@ -752,72 +802,51 @@ void DeviceSim::step(const SpawnRec *recs, int n) {
     Impl &I = *impl_;
     View &V = I.V;
     cudaStream_t s = I.stream;
-    const int TPB = 256;
-    const int gLaneRL = (std::max(V.nLanes, V.nRL) + TPB - 1) / TPB;
-    // list-driven kernels: fixed grids sized to the machine (grid-stride loops inside)
-    ensureGrids();   // one resident wave per kernel (occupancy x #SM blocks)
+    I.ensureGrids();
     const bool tm = I.timing;
-    auto launchAll = [&](bool withEvents) {
-        const bool pdl = I.usePdl && !withEvents;   // (events between the kernels would serialise them anyway)
-        if (withEvents) cudaEventRecord(I.ev[0], s);
-        launchPdl(k_ingest, std::max(gLaneRL, 1), TPB, s, false, V);   // follows a copy, not a kernel
-        if (withEvents) cudaEventRecord(I.ev[1], s);
-        launchPdl(k_notify, I.gridNotify, TPB, s, pdl, V);
-        if (withEvents) cudaEventRecord(I.ev[2], s);
-        launchPdl(k_control, I.gridControl, 256, s, pdl, V);
-        if (withEvents) cudaEventRecord(I.ev[3], s);
-        launchPdl(k_move, I.gridMove, TPB, s, pdl, V);
-        if (withEvents) cudaEventRecord(I.ev[4], s);
-        launchPdl(k_leader, I.gridLeader, TPB, s, pdl, V);
-        if (withEvents) cudaEventRecord(I.ev[5], s);
+    auto launchAll = [&]() {   // with kernel timing: an event before and after each kernel
+        for (int k = 0; k < 5; ++k) {
+            if (tm) cudaEventRecord(I.ev[k], s);
+            I.launchStep((Impl::StepKernel) k, I.pdl());
+        }
+        if (tm) cudaEventRecord(I.ev[5], s);
     };
     if (!tm && I.useCoop) {
         if (!I.gridStep) {
             int b = 0;
-            CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_step, TPB, 0));
+            CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_step, 256, 0));
             I.gridStep = std::max(b, 1) * I.numSMs;
         }
         void *args[] = {(void *) &V};
-        CFB_CUDA(cudaLaunchCooperativeKernel((void *) k_step, dim3(I.gridStep), dim3(TPB), args, 0, s));
+        CFB_CUDA(cudaLaunchCooperativeKernel((void *) k_step, dim3(I.gridStep), dim3(256), args, 0, s));
     } else if (tm || !I.useGraph) {
-        launchAll(tm);
+        launchAll();
     } else {
         // The five kernels of one step are replayed as one CUDA graph per list parity: one launch
         // call per step instead of five, and no host-paced gaps between the kernels.
-        if (I.graphDirty) {
-            I.dropGraphs();
-            I.graphDirty = false;
-        }
-        const int ring = (int) ((steps_ >> 1) % Impl::GRING);
-        cudaGraphExec_t &ge = I.graphExec[V.par][ring];
-        if (!ge) {
-            cudaGraph_t &g = I.graphTemplate[V.par];
-            for (int attempt = 0; attempt < 2 && !ge; ++attempt) {
-                if (!g) {
-                    CFB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-                    launchAll(false);
-                    if (cudaStreamEndCapture(s, &g) != cudaSuccess) g = nullptr;
-                }
-                if (!g || cudaGraphInstantiate(&ge, g, 0) != cudaSuccess) {
-                    // a driver that cannot put programmatic dependencies into a graph: plain edges instead
-                    cudaGetLastError();
-                    if (g) { cudaGraphDestroy(g); g = nullptr; }
-                    ge = nullptr;
-                    if (!I.usePdl) throw std::runtime_error("cityflow_b200: cannot capture the step into a CUDA graph");
-                    I.usePdl = false;
-                }
+        GraphRing &G = I.graphs;
+        const int r = GraphRing::slot(steps_);
+        cudaGraphExec_t &ge = G.exec[V.par][r];
+        cudaGraph_t &g = G.tmpl[V.par];
+        for (int attempt = 0; attempt < 2 && !ge; ++attempt) {
+            if (!g) {
+                CFB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+                launchAll();
+                if (cudaStreamEndCapture(s, &g) != cudaSuccess) g = nullptr;
+            }
+            if (!g || !G.instantiate(V.par, r)) {
+                // a driver that cannot put programmatic dependencies into a graph: plain edges instead
+                cudaGetLastError();
+                if (g) { cudaGraphDestroy(g); g = nullptr; }
+                ge = nullptr;
+                if (!I.usePdl) throw std::runtime_error("cityflow_b200: cannot capture the step into a CUDA graph");
+                I.usePdl = false;
             }
         }
-        // Re-launching an executable graph whose previous launch has not finished makes the driver
-        // wait on the host (observed: ~1 ms per step), hence the ring of instances; when even the ring
-        // is exhausted fall back to the five plain launches, which only enqueue.
-        cudaEvent_t &done = I.graphDone[V.par][ring];
-        if (!done) CFB_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-        else if (cudaEventQuery(done) != cudaSuccess) { launchAll(false); goto launched; }
-        CFB_CUDA(cudaGraphLaunch(ge, s));
-        CFB_CUDA(cudaEventRecord(done, s));
+        // when even the ring is exhausted: the five plain launches, which only enqueue
+        if (G.busy(V.par, r)) launchAll();
+        else G.launch(V.par, r, s);
     }
-launched:
     CFB_CUDA(cudaGetLastError());
     {   // (a graph step that found its ring instance busy and launched plainly still counts as the graph form)
         const bool coop = !tm && I.useCoop;
@@ -844,8 +873,7 @@ static void readCtrlImpl(cudaStream_t s, Ctrl *dst, const Ctrl *src);
 void DeviceSim::synchronize() { CFB_CUDA(cudaStreamSynchronize(impl_->stream)); }
 
 // ------------------------------------------------------------------------------------------
-// Sharded mode (partition.h / shard.h): the step is run phase by phase, with the seam exchanges
-// (performed by a ShardTransport on this engine's stream) in between.
+// Sharded mode (partition.h / shard.h): the step with the seam exchanges in between (Impl::shardKernels).
 void DeviceSim::configureShard(int rank, int world, const std::vector<unsigned char> &owned,
                                const std::vector<std::vector<int>> &feedPerPeer,
                                const std::vector<std::vector<int>> &ownPerPeer,
@@ -887,75 +915,43 @@ ShardBuffers DeviceSim::shardBuffers() {
     Impl &I = *impl_;
     ShardBuffers b;
     b.stream = (void *) I.stream;
-    b.rank = I.shardRank;
-    b.world = I.shardWorld;
     b.tailSend = I.tailSend.p; b.tailRecv = I.tailRecv.p; b.moverSend = I.moverSend.p; b.moverRecv = I.moverRecv.p;
     b.tailBytes = sizeof(TailMsg); b.moverBytes = sizeof(MoverMsg);
     b.outBeg = I.outBeg; b.inBeg = I.inBeg;
     b.blkSend = I.blkUpd.p; b.blkAll = I.blkAll.p;
     b.blkBytesPerRank = (size_t) (1 + I.V.blkUpdCap) * sizeof(int2);
-    b.ctrlActive = &I.V.ctrl->active;
-    b.laneCount = I.V.count;
     return b;
 }
 
-void DeviceSim::runIngest() {
+// One step of one rank of a multi-process run (see Impl::shardKernels for the kernel sequence).
+void DeviceSim::shardStep(const SpawnRec *recs, int n, ShardTransport *t) {
     Impl &I = *impl_;
-    const int TPB = 256;
-    const int g = ((I.V.ingLanes ? std::max(std::max(I.V.nIngLanes, I.V.nIngRL), I.V.nIngLinks * I.V.maskWords / 4) : std::max(I.V.nLanes, I.V.nRL)) + TPB - 1) / TPB;
-    k_ingest<<<std::max(g, 1), TPB, 0, I.stream>>>(I.V);
-    launches_ += 1;
+    stageStep(recs, n);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        const int st = I.shardGraphBegin(steps_);
+        if (st != 1) try {
+            I.shardKernels(t, launches_);
+        } catch (const std::exception &) {
+            if (st != 2 || I.p2p) throw;
+            // a staged exchange refused to be captured: abandon the graph, run this step plainly
+        }
+        if (I.shardGraphEnd(st, steps_)) break;
+    }
+    CFB_CUDA(cudaGetLastError());
+    steps_ += 1;
+    I.epochHost += 1;
 }
-void DeviceSim::runNotifyControl() {
+
+void DeviceSim::shardSegment(int k) {
     Impl &I = *impl_;
-    ensureGrids();
-    launchPdl(k_notify, I.gridNotify, 256, I.stream, I.usePdl && !I.timing, I.V);   // behind k_ingest
-    launchPdl(k_control, I.gridControl, 256, I.stream, I.usePdl && !I.timing, I.V);
-    launches_ += 2;
+    I.shardSegment(k, false, launches_);
+    if (k == 2) {
+        CFB_CUDA(cudaGetLastError());
+        steps_ += 1;
+        I.epochHost += 1;
+    }
 }
-void DeviceSim::runMove() {
-    Impl &I = *impl_;
-    ensureGrids();
-    launchPdl(k_move, I.gridMove, 256, I.stream, I.usePdl && !I.timing, I.V);
-    launches_ += 1;
-}
-void DeviceSim::runLeader() {
-    Impl &I = *impl_;
-    ensureGrids();
-    launchPdl(k_leader, I.gridLeader, 256, I.stream, I.usePdl && !I.timing, I.V);
-    launches_ += 1;
-}
-void DeviceSim::packTails() {
-    Impl &I = *impl_;
-    if (I.V.nBoundIn) k_pack_tails<<<(I.V.nBoundIn + 127) / 128, 128, 0, I.stream>>>(I.V, I.tailSend.p);
-    launches_ += 1;
-}
-void DeviceSim::unpackTails() {
-    Impl &I = *impl_;
-    if (I.V.nBoundOut) k_unpack_tails<<<(I.V.nBoundOut + 127) / 128, 128, 0, I.stream>>>(I.V, I.tailRecv.p);
-    launches_ += 1;
-}
-void DeviceSim::packMovers() {
-    Impl &I = *impl_;
-    if (I.V.nBoundOut) k_pack_movers<<<(I.V.nBoundOut * 32 + 127) / 128, 128, 0, I.stream>>>(I.V, I.moverSend.p);
-    launches_ += 1;
-}
-void DeviceSim::unpackMovers() {
-    Impl &I = *impl_;
-    if (I.V.nBoundIn) k_unpack_movers<<<(I.V.nBoundIn * 32 + 127) / 128, 128, 0, I.stream>>>(I.V, I.moverRecv.p);
-    launches_ += 1;
-}
-void DeviceSim::sealBlk() {
-    Impl &I = *impl_;
-    k_seal_blk<<<1, 1, 0, I.stream>>>(I.V);
-    launches_ += 1;
-}
-void DeviceSim::applyBlk() {
-    Impl &I = *impl_;
-    dim3 grid(32, I.shardWorld);
-    k_apply_blk<<<grid, 256, 0, I.stream>>>(I.V, I.blkAll.p, I.shardWorld, I.shardRank, 1 + I.V.blkUpdCap);
-    launches_ += 1;
-}
+
 // ---- peer-memory transport (device_shard.cuh) ----
 // The arena other ranks write into.  From here on the slot-indexed arrays have their final size (delStep lives in
 // the arena and is mapped by the peers).
@@ -972,8 +968,7 @@ DeviceSim::ShardArena DeviceSim::shardArena() {
         legacySync();
         I.delStep.release();
         I.V.delStep = (int *) (I.arena.p + L.delStep);
-        I.graphDirty = true;
-        I.dropShardGraphs();
+        I.invalidateGraphs();
     }
     return ShardArena{I.arena.p, I.arena.n};
 }
@@ -1017,44 +1012,8 @@ void DeviceSim::shardConnect(const std::vector<void *> &peerBase) {
     if (V.blkUpdCap > BLK_IN_CAP) V.blkUpdCap = BLK_IN_CAP;
     if (const char *g = getenv("CITYFLOW_B200_SHARD_SPLIT")) I.shardSplit = g[0] == '1';
     I.p2p = true;
-    I.dropShardGraphs();
+    I.invalidateGraphs();
     legacySync();
-}
-bool DeviceSim::shardIsP2P() const { return impl_->p2p; }
-
-void DeviceSim::sendMovers() {
-    Impl &I = *impl_;
-    const int g = std::max(1, std::min(64, (I.V.nBoundOut * 32 + 127) / 128));
-    launchPdl(k_send_movers, g, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
-}
-void DeviceSim::recvMovers() {
-    Impl &I = *impl_;
-    const int g = std::max(1, std::min(64, (I.V.nBoundIn * 32 + 127) / 128));
-    launchPdl(k_recv_movers, g, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
-}
-void DeviceSim::xchgMovers() {
-    Impl &I = *impl_;
-    const int g = std::max(1, std::min(64, (std::max(I.V.nBoundOut, I.V.nBoundIn) * 32 + 127) / 128));
-    launchPdl(k_xchg_movers, g, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
-}
-void DeviceSim::xchgTails() {
-    Impl &I = *impl_;
-    launchPdl(k_xchg_tails, 16, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
-}
-bool DeviceSim::shardSplitKernels() const { return impl_->shardSplit || impl_->timing; }
-void DeviceSim::sendTails() {
-    Impl &I = *impl_;
-    launchPdl(k_send_tails, 16, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
-}
-void DeviceSim::recvTails() {
-    Impl &I = *impl_;
-    launchPdl(k_recv_tails, 16, 128, I.stream, I.usePdl && !I.timing, I.V, I.S);
-    launches_ += 1;
 }
 
 // Network-wide vehicle count over the peer-memory arena (k_sum_active); false: not available, use shardCounts().
@@ -1124,72 +1083,6 @@ void DeviceSim::shardGatherFinished(ShardTransport *t, std::vector<FinRec> &inou
     }
 }
 
-// One sharded step (kernels + NCCL operations enqueued by the caller between begin and end) is
-// captured into a CUDA graph per list parity and replayed: one launch call per step instead of ~17.
-// The first steps run uncaptured so that NCCL can set up its connections; any capture failure
-// switches the engine back to plain launches for good.
-int DeviceSim::shardStepBegin() {
-    Impl &I = *impl_;
-    const int par = I.V.par;
-    if (!I.shardGraphOk || steps_ < 8 || I.timing) return 0;           // plain
-    const int ring = (int) ((steps_ >> 1) % Impl::GRING);
-    cudaGraphExec_t &ge = I.shardGraph[par][ring];
-    cudaEvent_t &done = I.shardGraphDone[par][ring];
-    if (!done) CFB_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-    if (ge || I.shardTemplate[par]) {
-        if (!ge && cudaGraphInstantiate(&ge, I.shardTemplate[par], 0) != cudaSuccess) { cudaGetLastError(); ge = nullptr; return 0; }
-        else if (cudaEventQuery(done) != cudaSuccess) { cudaGetLastError(); return 0; }   // this instance is still running: just enqueue
-        CFB_CUDA(cudaGraphLaunch(ge, I.stream));
-        CFB_CUDA(cudaEventRecord(done, I.stream));
-        return 1;                                                     // replayed: the caller skips the phases
-    }
-    if (cudaStreamBeginCapture(I.stream, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
-        cudaGetLastError();
-        I.shardGraphOk = false;
-        return 0;
-    }
-    return 2;                                                         // capturing: the caller enqueues the phases
-}
-
-bool DeviceSim::shardStepEnd(int state) {
-    Impl &I = *impl_;
-    bool ok = true;
-    if (state == 2) {
-        const int par = I.V.par;
-        const int ring = (int) ((steps_ >> 1) % Impl::GRING);
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamEndCapture(I.stream, &g);
-        if (e == cudaSuccess && g) e = cudaGraphInstantiate(&I.shardGraph[par][ring], g, 0);
-        if (e != cudaSuccess || !I.shardGraph[par][ring]) {
-            if (g) cudaGraphDestroy(g);
-            cudaGetLastError();
-            I.shardGraph[par][ring] = nullptr;
-            I.shardGraphOk = false;
-            ok = false;                                                // nothing ran: the caller repeats the step plainly
-        } else {
-            I.shardTemplate[par] = g;
-            CFB_CUDA(cudaGraphLaunch(I.shardGraph[par][ring], I.stream));
-            CFB_CUDA(cudaEventRecord(I.shardGraphDone[par][ring], I.stream));
-        }
-    }
-    if (ok) {
-        CFB_CUDA(cudaGetLastError());
-        steps_ += 1;
-        I.epochHost += 1;
-    }
-    return ok;
-}
-
-void DeviceSim::ensureGrids() {
-    Impl &I = *impl_;
-    if (I.gridNotify) return;
-    int b = 0;
-    CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_notify, 256, 0)); I.gridNotify = std::max(b, 1) * I.numSMs;
-    CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_move, 256, 0)); I.gridMove = std::max(b, 1) * I.numSMs;
-    CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_leader, 256, 0)); I.gridLeader = std::max(b, 1) * I.numSMs;
-    CFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_control, 256, 0)); I.gridControl = std::max(b, 1) * I.numSMs;
-}
-
 // ---- measurement support: CUDA-event brackets on the engine's own stream ----
 void DeviceSim::flushL2() {
     Impl &I = *impl_;
@@ -1256,25 +1149,7 @@ void DeviceSim::enableKernelTiming(bool on) {
     for (double &x : impl_->shardMs) x = 0;
     impl_->shardTimedSteps = 0;
 }
-bool DeviceSim::timingOn() const { return impl_->timing; }
-void DeviceSim::shardTimeMark(int k) {
-    Impl &I = *impl_;
-    if (!I.timing) return;
-    if (!I.shardEv[k]) CFB_CUDA(cudaEventCreate(&I.shardEv[k]));
-    CFB_CUDA(cudaEventRecord(I.shardEv[k], I.stream));
-}
-void DeviceSim::shardTimeCollect() {
-    Impl &I = *impl_;
-    if (!I.timing) return;
-    CFB_CUDA(cudaEventSynchronize(I.shardEv[SHARD_PHASES]));
-    for (int k = 0; k < SHARD_PHASES; ++k) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, I.shardEv[k], I.shardEv[k + 1]);
-        I.shardMs[k] += ms;
-    }
-    I.shardTimedSteps += 1;
-}
-void DeviceSim::shardPhaseTimes(double ms[SHARD_PHASES], long long *steps) {
+void DeviceSim::shardStepTimes(double ms[SHARD_PHASES], long long *steps) {
     for (int k = 0; k < SHARD_PHASES; ++k) ms[k] = impl_->shardMs[k];
     if (steps) *steps = impl_->shardTimedSteps;
 }
@@ -1727,7 +1602,7 @@ void DeviceSim::stepLcBegin(const SpawnRec *recs, int n, const int32_t *spare, i
     View &V = I.V;
     cudaStream_t s = I.stream;
     const int TPB = 256;
-    ensureGrids();
+    I.ensureGrids();
     if (nSpare > I.lcSpareCap) {
         CFB_CUDA(cudaStreamSynchronize(s));
         I.lcSpareCap = std::max(1024, nSpare * 2);
@@ -1736,9 +1611,8 @@ void DeviceSim::stepLcBegin(const SpawnRec *recs, int n, const int32_t *spare, i
     if (nSpare > 0) CFB_CUDA(cudaMemcpyAsync(I.lcSpare.p, spare, nSpare * sizeof(int), cudaMemcpyHostToDevice, s));
     V.lc.spare = I.lcSpare.p;
     V.lc.nSpare = nSpare;
-    const int gLaneRL = (std::max(V.nLanes, V.nRL) + TPB - 1) / TPB;
     k_lc_begin<<<1, 1, 0, s>>>(V.lc);
-    k_ingest<<<std::max(gLaneRL, 1), TPB, 0, s>>>(V);
+    I.launchStep(Impl::INGEST, false);
     k_lc_admitted<<<I.gridNotify, TPB, 0, s>>>(V, V.lc);
     k_lc_segments<<<I.gridNotify, TPB, 0, s>>>(V, V.lc);
     k_lc_signal<<<I.gridControl, TPB, 0, s>>>(V, V.lc);
@@ -1773,8 +1647,8 @@ void DeviceSim::stepLcEnd(const int32_t *priorities, int n) {
         k_lc_priorities<<<(n + 127) / 128, 128, 0, s>>>(V, V.lc, I.lcPrio.p, n);
     }
     k_lc_leader<<<I.gridNotify, TPB, 0, s>>>(V, V.lc);
-    k_notify<<<I.gridNotify, TPB, 0, s>>>(V);
-    k_control<<<I.gridControl, 256, 0, s>>>(V);
+    I.launchStep(Impl::NOTIFY, false);
+    I.launchStep(Impl::CONTROL, false);
     if (I.lcSerial) {
         k_lc_control_tail<<<1, 32, 0, s>>>(V, V.lc);
     } else {
@@ -1782,8 +1656,8 @@ void DeviceSim::stepLcEnd(const int32_t *priorities, int n) {
         k_lc_tail_roads<<<LC_MAX_CAND / 128, 128, 0, s>>>(V, V.lc);
         k_lc_tail_clear<<<1, 32, 0, s>>>(V, V.lc);
     }
-    k_move<<<I.gridMove, TPB, 0, s>>>(V);
-    k_leader<<<I.gridLeader, TPB, 0, s>>>(V);
+    I.launchStep(Impl::MOVE, false);
+    I.launchStep(Impl::LEADER, false);
     CFB_CUDA(cudaGetLastError());
     launches_ += 6 + (n > 0);
     steps_ += 1;

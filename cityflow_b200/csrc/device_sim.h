@@ -85,20 +85,17 @@ struct DeviceSimOptions {
     int replicas = 1;           // bench only: K independent copies of the scenario in one engine
 };
 
-// Device buffers a ShardTransport moves between ranks (all on `stream`).  Per peer q the tail /
-// mover messages of the lanes shared with q are contiguous: entries [beg[q], beg[q+1]).
+// The staged exchange's device buffers (all on `stream`), for a caller of shardSegment that moves them itself.  Per peer
+// q the tail / mover messages of the lanes shared with q are contiguous: entries [beg[q], beg[q+1]).
 class ShardTransport;
 
 struct ShardBuffers {
     void *stream = nullptr;
-    int rank = 0, world = 1;
     void *tailSend = nullptr, *tailRecv = nullptr, *moverSend = nullptr, *moverRecv = nullptr;
     size_t tailBytes = 0, moverBytes = 0;       // bytes per boundary lane
     std::vector<int> outBeg, inBeg;             // lanes this rank feeds / owns, per peer (prefix sums)
     void *blkSend = nullptr, *blkAll = nullptr; // blocker changes: own list, all ranks' lists
     size_t blkBytesPerRank = 0;
-    int *ctrlActive = nullptr;                  // device int: vehicles this rank accounts for
-    int *laneCount = nullptr;                   // device ints: list length per drivable
 };
 
 struct DeviceObs {
@@ -126,7 +123,7 @@ public:
     void uploadPlans(const Routing &routing);
     void ensureSlotCapacity(int slots);
 
-    // ---- sharded mode: the step phase by phase (see shard.h for the protocol) ----
+    // ---- sharded mode (see shard.h for the protocol) ----
     void configureShard(int rank, int world, const std::vector<unsigned char> &owned,
                         const std::vector<std::vector<int>> &feedPerPeer, const std::vector<std::vector<int>> &ownPerPeer,
                         const std::vector<std::vector<int>> &boundarySize, const std::vector<unsigned char> &ownedRoadLinks);
@@ -135,28 +132,17 @@ public:
     ShardArena shardArena();
     void shardConnect(const std::vector<void *> &peerBase);
     void shardMarkArenaExported();   // other processes map the arena: it must outlive them (never freed)
-    bool shardIsP2P() const;
-    void sendMovers();
-    void recvMovers();
-    void sendTails();
-    void recvTails();
-    void xchgMovers();               // send + receive in one kernel (default)
-    void xchgTails();
-    bool shardSplitKernels() const;
-    ShardBuffers shardBuffers();
+    // One step of one rank of a multi-process run (asynchronous): the whole kernel sequence with both seam exchanges,
+    // over peer memory once connected, else staged through `t`; replayed as a CUDA graph from the ninth step on.
+    void shardStep(const SpawnRec *recs, int n, ShardTransport *t);
+    // The same step for a caller that moves the seam records itself (the loop-back group): stageStep, then segment k =
+    //   0  ingest, notify, control, send (peer memory) or pack the movers
+    //   1  receive or unpack the movers, move, send or pack the tails and seal the blocker list
+    //   2  receive or unpack the tails, apply the blocker lists, leader; counts the step
+    // with the movers' exchange between 0 and 1, and the tails' and blocker lists' between 1 and 2.
     void stageStep(const SpawnRec *recs, int n);
-    int shardStepBegin();            // 0 plain, 1 replayed (skip the phases), 2 capturing
-    bool shardStepEnd(int state);    // false: capture failed, nothing ran -> repeat the phases plainly
-    void runIngest();
-    void runNotifyControl();
-    void runMove();
-    void runLeader();
-    void packTails();
-    void unpackTails();
-    void packMovers();
-    void unpackMovers();
-    void sealBlk();
-    void applyBlk();
+    void shardSegment(int k);
+    ShardBuffers shardBuffers();     // what the staged exchanges move
     void shardCounts(ShardTransport *t, int32_t *laneOut, int *activeOut);   // global sums (collective)
     bool shardVehicleCount(int *activeOut);        // the same count over the peer-memory arena (no all-reduce); false = unavailable
     void shardWaitingCounts(ShardTransport *t, int32_t *laneOut);
@@ -215,10 +201,7 @@ public:
     void enableKernelTiming(bool on);
     // sharded step, phase by phase: ingest | notify+control | send movers | recv movers | move | send tails | recv tails | leader
     static constexpr int SHARD_PHASES = 8;
-    bool timingOn() const;
-    void shardTimeMark(int k);                       // records event k (0..SHARD_PHASES) when timing is on
-    void shardTimeCollect();                         // after mark SHARD_PHASES: accumulates the phase durations
-    void shardPhaseTimes(double ms[SHARD_PHASES], long long *steps);
+    void shardStepTimes(double ms[SHARD_PHASES], long long *steps);
     void flushL2();                 // 256 MiB memset on the engine stream
     void markTimed();               // record an event; brackets are (even, odd) pairs
     double collectTimedMs();        // sync; sum of bracket durations; clears the brackets
@@ -255,7 +238,6 @@ public:
     struct Impl;
 
 private:
-    void ensureGrids();
     Impl *impl_;
     long long steps_ = 0;
     long long launches_ = 0;

@@ -676,13 +676,6 @@ public:
         step += 1;
         if ((step & 255) == 0) drain();  // bound the finished ring / free slots in long unobserved runs
     }
-    // device phases up to (not including) the exchange points; see shard.h
-    void shardPhase(int k) {
-        switch (k) {
-            case 2: dev->unpackMovers(); dev->runMove(); dev->packTails(); dev->sealBlk(); break;
-            case 3: dev->unpackTails(); dev->applyBlk(); dev->runLeader(); break;
-        }
-    }
     // One step with lane change: the shadows' priorities come from the engine RNG right after
     // this step's spawn draws (vehicle.cpp:33), so the step has a host round trip in the middle.
     void nextStepLaneChange() {
@@ -720,60 +713,8 @@ public:
         if (!ahead) prepareStep();
         ahead = false;
         const auto t1 = std::chrono::steady_clock::now();
-        if (!transport) {
-            dev->step(batch.data(), (int) batch.size());
-        } else {  // one rank of a sharded run: phases with the seam exchanges in between
-            dev->stageStep(batch.data(), (int) batch.size());
-            for (int attempt = 0; attempt < 2; ++attempt) {
-                const int st = dev->shardStepBegin();
-                if (st != 1 && dev->shardIsP2P()) {
-                    // peer-memory data plane (device_shard.cuh): the seam records are stored straight into the
-                    // neighbours' mailboxes by the send kernels; nothing but kernels on the stream
-                    const bool split = dev->shardSplitKernels();
-                    if (!split) {   // 7 kernels: ingest, notify, control, exchange movers, move, exchange tails, leader
-                        dev->runIngest();
-                        dev->runNotifyControl();
-                        dev->xchgMovers();                                                                 // X1
-                        dev->runMove();
-                        dev->xchgTails();                                                                  // X2
-                        dev->runLeader();
-                    } else {
-                    dev->shardTimeMark(0);
-                    dev->runIngest();
-                    dev->shardTimeMark(1);
-                    dev->runNotifyControl();
-                    dev->shardTimeMark(2);
-                    dev->sendMovers();                                                                     // X1
-                    dev->shardTimeMark(3);
-                    dev->recvMovers();
-                    dev->shardTimeMark(4);
-                    dev->runMove();
-                    dev->shardTimeMark(5);
-                    dev->sendTails();                                                                      // X2
-                    dev->shardTimeMark(6);
-                    dev->recvTails();
-                    dev->shardTimeMark(7);
-                    dev->runLeader();
-                    dev->shardTimeMark(8);
-                    dev->shardTimeCollect();
-                    }
-                } else if (st != 1) try {
-                    ShardBuffers b = dev->shardBuffers();
-                    dev->runIngest();
-                    dev->runNotifyControl();
-                    dev->packMovers();
-                    transport->exchange(b.stream, b.moverSend, b.outBeg, b.moverRecv, b.inBeg, b.moverBytes);  // X1
-                    shardPhase(2);
-                    transport->exchangeAndGather(b.stream, b.tailSend, b.inBeg, b.tailRecv, b.outBeg, b.tailBytes,
-                                                 b.blkSend, b.blkAll, b.blkBytesPerRank);                      // X2
-                    shardPhase(3);
-                } catch (const std::exception &) {
-                    if (st != 2) throw;
-                    // an operation refused to be captured: abandon the graph, run this step plainly
-                }
-                if (dev->shardStepEnd(st)) break;
-            }
-        }
+        if (!transport) dev->step(batch.data(), (int) batch.size());
+        else dev->shardStep(batch.data(), (int) batch.size(), transport);   // one rank of a sharded run
         hostEnqueueNs += std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t1).count();
         finishStep();
         prepareAhead();
@@ -1655,7 +1596,7 @@ int cfb_kernel_times(cfb_engine *e, double ms[5], int64_t *steps) {
 }
 int cfb_shard_phase_times(cfb_engine *e, double ms[8], int64_t *steps) {
     long long n = 0;
-    e->h.dev->shardPhaseTimes(ms, &n);
+    e->h.dev->shardStepTimes(ms, &n);
     if (steps) *steps = n;
     return CFB_OK;
 }
@@ -2161,24 +2102,23 @@ int cfb_shard_group_step(cfb_shard_group *g, int n) {
         const int W = (int) g->ranks.size();
         for (int it = 0; it < n; ++it) {
             std::vector<cfb::ShardBuffers> B;
-            for (auto *e : g->ranks) { e->h.prepareStep(); B.push_back(e->h.dev->shardBuffers()); }
-            for (auto *e : g->ranks) { e->h.dev->stageStep(e->h.batch.data(), (int) e->h.batch.size()); e->h.dev->runIngest(); }
-            if (g->p2p) {
-                // the ranks' streams are drained between the phases, so a receive kernel never has to spin here:
-                // what this checks is the protocol (indices, parities, epochs), not the waiting
-                auto syncAll = [&]() { for (auto *e : g->ranks) e->h.dev->synchronize(); };
-                for (auto *e : g->ranks) { e->h.dev->runNotifyControl(); e->h.dev->sendMovers(); }
-                syncAll();
-                for (auto *e : g->ranks) { e->h.dev->recvMovers(); e->h.dev->runMove(); e->h.dev->sendTails(); }
-                syncAll();
-                for (auto *e : g->ranks) { e->h.dev->recvTails(); e->h.dev->runLeader(); e->h.dev->shardStepEnd(0); }
-            } else {
-                for (auto *e : g->ranks) { e->h.dev->runNotifyControl(); e->h.dev->packMovers(); }
-                loopExchange(B, false);
-                for (auto *e : g->ranks) e->h.shardPhase(2);
-                loopExchange(B, true);
-                loopAllGatherBlk(B);
-                for (auto *e : g->ranks) { e->h.shardPhase(3); e->h.dev->shardStepEnd(0); }
+            for (auto *e : g->ranks) {
+                e->h.prepareStep();
+                e->h.dev->stageStep(e->h.batch.data(), (int) e->h.batch.size());
+                B.push_back(e->h.dev->shardBuffers());
+            }
+            // Between the segments the ranks' streams are drained.  Over peer memory a receive kernel then never has to
+            // spin: what this checks is the protocol (indices, parities, epochs), not the waiting.
+            for (int k = 0; k < 3; ++k) {
+                if (k > 0) {
+                    if (g->p2p) {
+                        for (auto *e : g->ranks) e->h.dev->synchronize();
+                    } else {
+                        loopExchange(B, k == 2);
+                        if (k == 2) loopAllGatherBlk(B);
+                    }
+                }
+                for (auto *e : g->ranks) e->h.dev->shardSegment(k);
             }
             for (int r = 0; r < W; ++r) g->ranks[r]->h.finishStep();   // rank 0 first: its drain collects all lists
         }

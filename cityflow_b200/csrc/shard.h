@@ -1,7 +1,8 @@
 // Multi-GPU execution of one simulation: one process per GPU, the road graph cut by intersection
 // (partition.h), the seam records exchanged on the engine's CUDA stream.
 //
-// Per step and rank (DeviceSim phase API):
+// Per step and rank (DeviceSim::shardStep; DeviceSim::shardSegment runs the same sequence in three pieces, cut at
+// X1 and X2, for a caller that moves the records itself):
 //   stage + k_ingest                       admission into owned lanes -- and, identically, into the ghost
 //                                          copies of the lanes this rank feeds (so no exchange is needed here)
 //   k_notify, k_control

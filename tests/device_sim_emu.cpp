@@ -307,40 +307,35 @@ void DeviceSim::shardConnect(const std::vector<void *> &peerBase) {
     S.flags = E.flags.p(); S.blkIn = E.blkIn.p(); S.moverIn = E.moverIn.p(); S.tailIn = E.tailIn.p();
     E.connected = true;
 }
-bool DeviceSim::shardIsP2P() const { auto it = g_shardEmu.find(this); return it != g_shardEmu.end() && it->second.connected; }
 bool DeviceSim::shardVehicleCount(int *) { return false; }
-bool DeviceSim::timingOn() const { return false; }
 void DeviceSim::launchForm(int out[4]) const { for (int k = 0; k < 4; ++k) out[k] = 0; }   // no graph, no PDL, no grid, no mirror
 void DeviceSim::stepGrids(int out[5]) const { for (int k = 0; k < 4; ++k) out[k] = G; out[4] = 0; }
-void DeviceSim::shardTimeMark(int) {}
-void DeviceSim::shardTimeCollect() {}
-void DeviceSim::shardPhaseTimes(double *ms, long long *steps) { for (int k = 0; k < SHARD_PHASES; ++k) ms[k] = 0; if (steps) *steps = 0; }
+void DeviceSim::shardStepTimes(double *ms, long long *steps) { for (int k = 0; k < SHARD_PHASES; ++k) ms[k] = 0; if (steps) *steps = 0; }
 void DeviceSim::shardMarkArenaExported() {}
-void DeviceSim::sendMovers() { ShardEmu &E = g_shardEmu[this]; impl_->H.run(G, [&](int, int) { sendMoversBody(impl_->H.V, E.S); }); launches_ += 1; }
-void DeviceSim::recvMovers() { ShardEmu &E = g_shardEmu[this]; impl_->H.run(G, [&](int, int) { recvMoversBody(impl_->H.V, E.S); }); launches_ += 1; }
-void DeviceSim::sendTails() { ShardEmu &E = g_shardEmu[this]; impl_->H.run(G, [&](int, int) { sendTailsBody(impl_->H.V, E.S); }); launches_ += 1; }
-void DeviceSim::recvTails() { ShardEmu &E = g_shardEmu[this]; impl_->H.run(G, [&](int, int) { recvTailsBody(impl_->H.V, E.S); }); launches_ += 1; }
-void DeviceSim::xchgMovers() { notEmulated("the one-kernel exchange (two ranks would have to run at once)"); }
-void DeviceSim::xchgTails() { notEmulated("the one-kernel exchange (two ranks would have to run at once)"); }
-bool DeviceSim::shardSplitKernels() const { return true; }
-ShardBuffers DeviceSim::shardBuffers() { ShardBuffers b; b.rank = g_shardEmu[this].rank; b.world = g_shardEmu[this].world; return b; }
-int DeviceSim::shardStepBegin() { return 0; }
-bool DeviceSim::shardStepEnd(int) { steps_ += 1; return true; }
-void DeviceSim::runIngest() { HostSim &H = impl_->H; H.run(G, [&](int b, int nb) { phase_ingest(H.V, b, nb); }); launches_ += 1; }
-void DeviceSim::runNotifyControl() {
+// the peer-memory segments of the loop-back group, kernel for kernel as on the GPU
+void DeviceSim::shardSegment(int k) {
+    ShardEmu &E = g_shardEmu[this];
+    if (!E.connected) notEmulated("the staged (NCCL) seam exchange");
     HostSim &H = impl_->H;
-    H.run(G, [&](int b, int nb) { phase_notify(H.V, b, nb); });
-    H.run(G, [&](int b, int nb) { phase_control(H.V, b, nb); });
-    launches_ += 2;
+    View &V = H.V;
+    auto launch = [&](auto body) { H.run(G, body); launches_ += 1; };
+    if (k == 0) {
+        launch([&](int b, int nb) { phase_ingest(V, b, nb); });
+        launch([&](int b, int nb) { phase_notify(V, b, nb); });
+        launch([&](int b, int nb) { phase_control(V, b, nb); });
+        launch([&](int, int) { sendMoversBody(V, E.S); });
+    } else if (k == 1) {
+        launch([&](int, int) { recvMoversBody(V, E.S); });
+        launch([&](int b, int nb) { phase_move(V, b, nb); });
+        launch([&](int, int) { sendTailsBody(V, E.S); });
+    } else {
+        launch([&](int, int) { recvTailsBody(V, E.S); });
+        launch([&](int b, int nb) { phase_leader(V, b, nb); });
+        steps_ += 1;
+    }
 }
-void DeviceSim::runMove() { HostSim &H = impl_->H; H.run(G, [&](int b, int nb) { phase_move(H.V, b, nb); }); launches_ += 1; }
-void DeviceSim::runLeader() { HostSim &H = impl_->H; H.run(G, [&](int b, int nb) { phase_leader(H.V, b, nb); }); launches_ += 1; }
-void DeviceSim::packTails() { notEmulated("the staged (NCCL) seam exchange"); }
-void DeviceSim::unpackTails() { notEmulated("the staged (NCCL) seam exchange"); }
-void DeviceSim::packMovers() { notEmulated("the staged (NCCL) seam exchange"); }
-void DeviceSim::unpackMovers() { notEmulated("the staged (NCCL) seam exchange"); }
-void DeviceSim::sealBlk() { notEmulated("the staged (NCCL) seam exchange"); }
-void DeviceSim::applyBlk() { notEmulated("the staged (NCCL) seam exchange"); }
+void DeviceSim::shardStep(const SpawnRec *, int, ShardTransport *) { notEmulated("the multi-process sharded step"); }
+ShardBuffers DeviceSim::shardBuffers() { return ShardBuffers(); }
 void DeviceSim::shardCounts(ShardTransport *, int32_t *, int *) { notEmulated("sharding"); }
 void DeviceSim::shardWaitingCounts(ShardTransport *, int32_t *) { notEmulated("sharding"); }
 void DeviceSim::shardGatherFinished(ShardTransport *, std::vector<FinRec> &) { notEmulated("sharding"); }
@@ -407,6 +402,5 @@ double DeviceSim::collectTimedMs() { return 0; }
 void DeviceSim::debugCounters(unsigned long long out[8], bool) { for (int k = 0; k < 8; ++k) out[k] = 0; }
 int DeviceSim::debugArrays(unsigned *, unsigned *) { return 0; }
 DeviceSim::KernelTimes DeviceSim::kernelTimes() { return KernelTimes(); }
-void DeviceSim::ensureGrids() {}
 
 }  // namespace cfb
