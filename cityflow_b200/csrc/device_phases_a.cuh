@@ -191,7 +191,7 @@ __device__ __forceinline__ void phase_ingest(const View &V, const int bid, const
 }
 
 // ------------------------------------------------------------------------------------------
-// Cross::notify for one laneLink, executed by a whole warp: one lane per cross.
+// Cross::notify for one laneLink, executed by a 16-lane tile (half a warp): one lane per cross.
 // Engine::threadNotifyCross (engine.cpp:317-372) walks the link's crosses from the far end with
 // one cursor shared by three sources in order -- (1) the end lane's last vehicle if it came out
 // of this link, (2) the vehicles on the link front to back, (3) the start lane's first vehicle
@@ -199,65 +199,70 @@ __device__ __forceinline__ void phase_ingest(const View &V, const int bid, const
 // condition that is monotone along the link holds, so the owner of a cross is simply the first
 // source whose condition (same FP64 expression as the reference) holds for it.  Notify slots are
 // epoch-stamped instead of cleared (Cross::clearNotify would sweep every cross every step).
-__device__ void notifyLink(const View &V, int ll, int lane, int epoch) {
-    const int cb = V.llCrossBeg[ll], nc = V.llCrossBeg[ll + 1] - cb;
-    if (nc == 0) return;
+//
+// Both tiles of the warp call this together, each with its own link (`ll < 0`: none).  Every loop
+// around a shuffle runs to the larger trip count of the two tiles and predicates its work, so all 32
+// lanes meet at every warp primitive.
+__device__ void notifyLink(const View &V, const int ll, const int tl, const int epoch) {
+    int cb = 0, nc = 0, c2 = 0, base2 = 0;
+    int tp = -1, hp = -1;   // the owners sources 1 and 3 offer (-1: the source is absent)
+    double tdis = 0, vehDistance1 = 0, vehDistance3 = 0;
+    if (ll >= 0) {
+        cb = V.llCrossBeg[ll];
+        nc = V.llCrossBeg[ll + 1] - cb;
+    }
     const int linkDrv = V.nLanes + ll;
-    // source 1
-    bool has1 = false;
-    int tp = -1;
-    double tdis = 0, vehDistance1 = 0;
-    {
+    if (nc > 0) {
+        // source 1
         const Tail t = V.tail[V.llEndLane[ll]];
         if (t.pos >= 0 && t.prev == linkDrv) {
-            has1 = true;
             tp = t.pos;
             tdis = t.dis;
             vehDistance1 = tdis - t.len;
         }
-    }
-    // source 3
-    bool has3 = false;
-    int hp = -1;
-    double vehDistance3 = 0;
-    {
+        // source 3
         const int sl = V.llStartLane[ll];
         if (V.count[sl] > 0) {
-            hp = V.off[sl];
-            if (V.ids[hp].w == linkDrv && V.rlAvail[V.llRoadLink[ll]]) {
-                has3 = true;
-                vehDistance3 = V.drvLength[sl] - V.kin[hp].x;
+            const int h = V.off[sl];
+            if (V.ids[h].w == linkDrv && V.rlAvail[V.llRoadLink[ll]]) {
+                hp = h;
+                vehDistance3 = V.drvLength[sl] - V.kin[h].x;
             }
         }
+        c2 = V.count[linkDrv];
+        base2 = V.off[linkDrv];
+        if (tp < 0 && hp < 0 && c2 == 0) nc = 0;   // nothing to notify
     }
-    const int c2 = V.count[linkDrv], base2 = V.off[linkDrv];
-    if (!has1 && !has3 && c2 == 0) return;
-    const double L = V.drvLength[linkDrv];
-    const int linkW = V.linkInfo[ll].w;
-    for (int k0 = 0; k0 < nc; k0 += 32) {
-        const int k = k0 + lane;
+    if (nc == 0) c2 = 0;
+    const int tb = threadIdx.x & 16;   // the tile's first lane: shuffles read inside the caller's tile
+    const int ncMax = max(nc, __shfl_xor_sync(0xffffffffu, nc, 16));
+    const int c2Max = max(c2, __shfl_xor_sync(0xffffffffu, c2, 16));
+    const double L = nc > 0 ? V.drvLength[linkDrv] : 0.0;
+    const int linkW = nc > 0 ? V.linkInfo[ll].w : 0;
+    for (int k0 = 0; k0 < ncMax; k0 += 16) {
+        const int k = k0 + tl;
         const bool valid = k < nc;
         const double dk = valid ? V.lcDist[cb + k] : 0.0;
         int owner = -1;
         double ndist = 0;
-        if (valid && has1) {
+        if (valid && tp >= 0) {
             const double crossDistance = L - dk;
             if (crossDistance + vehDistance1 < 0) {
                 owner = tp;
                 ndist = -(tdis + crossDistance);
             }
         }
-        for (int j0 = 0; j0 < c2; j0 += 32) {  // vehicles on the link, front to back
+        for (int j0 = 0; j0 < c2Max; j0 += 16) {  // vehicles on the link, front to back
             double vj = 0, lj = 0;
-            if (j0 + lane < c2) {
-                vj = V.kin[base2 + j0 + lane].x;
-                lj = V.tmpl[V.ids[base2 + j0 + lane].y].len;
+            if (j0 + tl < c2) {
+                vj = V.kin[base2 + j0 + tl].x;
+                lj = V.tmpl[V.ids[base2 + j0 + tl].y].len;
             }
-            const int m = min(32, c2 - j0);
+            const int m = min(16, c2Max - j0);
             for (int j = 0; j < m; ++j) {
-                const double v = __shfl_sync(0xffffffffu, vj, j);
-                const double l = __shfl_sync(0xffffffffu, lj, j);
-                if (valid && owner < 0) {
+                const double v = __shfl_sync(0xffffffffu, vj, tb + j);
+                const double l = __shfl_sync(0xffffffffu, lj, tb + j);
+                if (valid && owner < 0 && j0 + j < c2) {
                     bool take = true;
                     if (v > dk) take = (v - dk - l <= 0);
                     if (take) {
@@ -267,7 +272,7 @@ __device__ void notifyLink(const View &V, int ll, int lane, int epoch) {
                 }
             }
         }
-        if (valid && owner < 0 && has3) {
+        if (valid && owner < 0 && hp >= 0) {
             owner = hp;
             ndist = vehDistance3 + dk;
         }
@@ -287,49 +292,58 @@ __device__ void notifyLink(const View &V, int ll, int lane, int epoch) {
     }
 }
 
-// k_notify: warp per occupied drivable.  A link handles itself; a lane triggers the (empty)
-// links its tail vehicle came out of / its head vehicle heads for, so no empty link is swept.
-// Also runs the leader search of a vehicle admitted to an empty lane this step.
+// k_notify: two occupied drivables per warp, one per 16-lane tile.  A link handles itself; a lane
+// triggers the (empty) links its tail vehicle came out of / its head vehicle heads for, so no empty
+// link is swept.  Also runs the leader search of a vehicle admitted to an empty lane this step.
+// Most laneLinks have at most 20 crosses and hold a few vehicles, so half a warp per link leaves
+// fewer lanes idle, and a resident wave of tiles covers the whole list in about one pass.
 __device__ __forceinline__ void phase_notify(const View &V, const int bid, const int nblk) {
-    const int lane = threadIdx.x & 31;
+    const int lane = threadIdx.x & 31, tile = lane >> 4, tl = lane & 15;
     const int warp = (bid * blockDim.x + threadIdx.x) >> 5;
     const int nWarps = (nblk * blockDim.x) >> 5;
     const int cpar = V.par;
     const int nAct = V.ctrl->nAct[cpar];
     const int epoch = V.ctrl->step + 1;
-    for (int w = warp; w < nAct; w += nWarps) {
-        const int d = V.actList[cpar][w];
-        if (d >= V.nLanes) {
-            notifyLink(V, d - V.nLanes, lane, epoch);
-            continue;
+    for (int w0 = 2 * warp; w0 < nAct; w0 += 2 * nWarps) {  // trip count uniform per warp
+        const int w = w0 + tile;
+        int la = -1, lb = -1;   // the links this tile notifies
+        if (w < nAct) {
+            const int d = V.actList[cpar][w];
+            if (d >= V.nLanes) {
+                la = d - V.nLanes;
+            } else if (V.count[d] > 0) {
+                const int c = V.count[d], base = V.off[d];
+                // with lane change the search already ran before the signals (k_lc_admitted) and the full leader
+                // pass after scheduling (k_lc_leader) has the final word
+                if ((V.inserted[d] & 2) && tl == 0 && !V.lcOn) {
+                    const int4 idv = V.ids[base];
+                    int ld = -1;
+                    double g = 0;
+                    headSearch(V, d, 0.0, idv.w, V.nav[base].x, V.tmpl[idv.y], d, ld, g);
+                    V.leader[base] = ld;
+                    if (ld >= 0) V.gap[base] = g;
+                    if (V.lcOn && ld >= 0) V.lc.slot[idv.x].gap = g;
+                }
+                // the link the tail came out of, if it is empty now (otherwise it is on the list itself)
+                const int prev = V.nav[base + c - 1].y;
+                if (prev >= V.nLanes && V.count[prev] == 0 && (!V.owned || V.owned[prev] == 1)) la = prev - V.nLanes;
+                // the link the head is about to take, if empty
+                const int nx = V.ids[base].w;
+                if (nx >= V.nLanes && V.count[nx] == 0 && nx - V.nLanes != la) lb = nx - V.nLanes;
+                if (la < 0) { la = lb; lb = -1; }
+            }
         }
-        const int c = V.count[d], base = V.off[d];
-        if (c == 0) continue;
-        // with lane change the search already ran before the signals (k_lc_admitted) and the full leader
-        // pass after scheduling (k_lc_leader) has the final word
-        if ((V.inserted[d] & 2) && lane == 0 && !V.lcOn) {
-            const int4 idv = V.ids[base];
-            int ld = -1;
-            double g = 0;
-            headSearch(V, d, 0.0, idv.w, V.nav[base].x, V.tmpl[idv.y], d, ld, g);
-            V.leader[base] = ld;
-            if (ld >= 0) V.gap[base] = g;
-            if (V.lcOn && ld >= 0) V.lc.slot[idv.x].gap = g;
-        }
-        // the link the tail came out of, if it is empty now (otherwise it is on the list itself)
-        const int prev = V.nav[base + c - 1].y;
-        int l1 = -1;
-        if (prev >= V.nLanes && V.count[prev] == 0 && (!V.owned || V.owned[prev] == 1)) {
-            l1 = prev - V.nLanes;
-            notifyLink(V, l1, lane, epoch);
-        }
-        // the link the head is about to take, if empty
-        const int nx = V.ids[base].w;
-        if (nx >= V.nLanes && V.count[nx] == 0 && nx - V.nLanes != l1) notifyLink(V, nx - V.nLanes, lane, epoch);
+        notifyLink(V, la, tl, epoch);
+        if (__ballot_sync(0xffffffffu, lb >= 0)) notifyLink(V, lb, tl, epoch);
     }
-    for (int w = warp; w < V.nBoundOut; w += nWarps) {  // sharded: source 1 may sit on a lane another rank owns
-        const Tail t = V.tail[V.boundOut[w]];
-        if (t.pos >= 0 && t.prev >= V.nLanes && V.owned[t.prev] == 1 && V.count[t.prev] == 0) notifyLink(V, t.prev - V.nLanes, lane, epoch);
+    for (int w0 = 2 * warp; w0 < V.nBoundOut; w0 += 2 * nWarps) {  // sharded: source 1 may sit on a lane another rank owns
+        const int w = w0 + tile;
+        int l = -1;
+        if (w < V.nBoundOut) {
+            const Tail t = V.tail[V.boundOut[w]];
+            if (t.pos >= 0 && t.prev >= V.nLanes && V.owned[t.prev] == 1 && V.count[t.prev] == 0) l = t.prev - V.nLanes;
+        }
+        notifyLink(V, l, tl, epoch);
     }
 }
 

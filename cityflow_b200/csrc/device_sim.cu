@@ -25,9 +25,9 @@
 // Kernel sequence per step (all FP64, -fmad=false so every operation rounds exactly like the
 // reference's SSE2 build; expression shapes follow vehicle.cpp verbatim):
 //   k_ingest   P0-P2  waiting-queue append, Lane::available admission, light -> roadLink mask
-//   k_notify   P3     Cross::notify, warp per occupied drivable, one lane per cross
+//   k_notify   P3     Cross::notify, half a warp (16-lane tile) per occupied drivable, one lane per cross
 //   k_control  P4     getNextSpeed / vehicleControl / setDeltaDistance, thread per vehicle
-//   k_move     P5-P6  bucket compaction (ballot scan), entrant rank-sort + append, commit,
+//   k_move     P5-P6  16-lane tile per drivable: bucket compaction (ballot scan), entrant rank-sort + append, commit,
 //                     finished ring, next step's work lists
 //   k_leader   P7-P8  leader/gap rebuild (warp shuffle), cross-drivable head search, blocker drop,
 //                     TrafficLight::passTime
