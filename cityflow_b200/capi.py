@@ -94,6 +94,7 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_debug_launch_form": (i32, [vp, vp]),
         "cfb_debug_step_grids": (i32, [vp, vp]),
         "cfb_shard_group_counters": (i32, [vp, vp]),
+        "cfb_debug_shard_group_create_cut": (vp, [cp, i32, i32, vp]),
     }
     for name, (res, args) in sig.items():
         if not hasattr(lib, name):
@@ -284,11 +285,19 @@ class CArchive:
 
 
 class CShardGroup:
-    """`world` ranks of one simulation on ONE GPU (loop-back exchanges): checks the seam protocol."""
+    """`world` ranks of one simulation on ONE GPU (loop-back exchanges): checks the seam protocol.  `owners`: the rank of
+    every intersection (virtual ones included), for a cut other than column strips."""
 
-    def __init__(self, config: str, world: int, device: int = 0):
-        self.lib = load_library()
-        self.h = self.lib.cfb_shard_group_create(config.encode(), world, device)
+    def _library(self) -> ctypes.CDLL:
+        return load_library()
+
+    def __init__(self, config: str, world: int, owners=None, device: int = 0):
+        self.lib = self._library()
+        if owners is None:
+            self.h = self.lib.cfb_shard_group_create(config.encode(), world, device)
+        else:
+            owners = np.ascontiguousarray(owners, np.int32)
+            self.h = self.lib.cfb_debug_shard_group_create_cut(config.encode(), world, device, owners.ctypes.data)
         if not self.h:
             raise RuntimeError("cfb_shard_group_create failed: %s" % self.lib.cfb_last_error(None).decode())
         self.world = world

@@ -747,13 +747,13 @@ public:
         batch.clear();
         idMapValid = false;
     }
-    // Cut the network and tell the device which part is ours (before the first step).
-    std::string configureShard(int rank, int world) {
+    // Tell the device which part of the cut `part` is ours (before the first step).
+    std::string configureShard(int rank, const Partition &part) {
         if (saveReplay) {
             std::cerr << "[cityflow_b200] saveReplay is not available on one rank of a sharded run; no replay is written" << std::endl;
             saveReplay = false;
         }
-        Partition part = Partition::columnStrips(net, world);
+        const int world = part.world;
         double look = 0;
         for (const auto &t : templates) look = std::max(look, t.maxSpeed * t.maxSpeed / t.usualNegAcc / 2 + t.maxSpeed * interval * 2);
         std::string bad = part.validate(net, look);
@@ -1953,7 +1953,7 @@ cfb_engine *cfb_engine_create_sharded(const char *config_file, int thread_num, i
     cfb_engine *e = cfb_engine_create(config_file, thread_num, device);
     if (!e || world <= 1) return e;
     DeviceGuard guard(e);
-    std::string err = e->h.configureShard(rank, world);
+    std::string err = e->h.configureShard(rank, cfb::Partition::columnStrips(e->h.net, world));
     if (err.empty()) e->transport.reset(cfb::createNcclTransport(rank, world, nccl_id, device < 0 ? 0 : device, err));
     if (!err.empty() || !e->transport) {
         g_createError = "sharded engine: " + err;
@@ -2008,6 +2008,7 @@ int cfb_shard_lane_vehicle_count(cfb_engine *e, int32_t *out, int n, int waiting
 // ---- loop-back group ----
 struct cfb_shard_group {
     std::vector<cfb_engine *> ranks;
+    cfb::Partition part;   // the cut every rank was configured with; the getters take lane owners from it
     std::string lastError;
     bool p2p = false;
 };
@@ -2053,14 +2054,33 @@ void loopAllGatherBlk(std::vector<cfb::ShardBuffers> &B) {
 
 extern "C" {
 
-cfb_shard_group *cfb_shard_group_create(const char *config_file, int world, int device) {
+// inter_owner: rank of every intersection (virtual ones included), or null for column strips
+static cfb_shard_group *shardGroupCreate(const char *config_file, int world, int device, const int32_t *inter_owner) {
     std::unique_ptr<cfb_shard_group> g(new cfb_shard_group());
+    auto fail = [&](const std::string &err) {
+        if (!err.empty()) g_createError = "sharded engine: " + err;
+        for (auto *x : g->ranks) cfb_engine_destroy(x);
+        return (cfb_shard_group *) nullptr;
+    };
     for (int r = 0; r < world; ++r) {
         cfb_engine *e = cfb_engine_create(config_file, 1, device);
-        if (!e) { for (auto *x : g->ranks) cfb_engine_destroy(x); return nullptr; }
+        if (!e) return fail("");
         g->ranks.push_back(e);
-        std::string err = e->h.configureShard(r, world);
-        if (!err.empty()) { g_createError = "sharded engine: " + err; for (auto *x : g->ranks) cfb_engine_destroy(x); return nullptr; }
+        if (r == 0) {
+            const cfb::RoadNet &net = e->h.net;
+            if (inter_owner) {
+                std::vector<int> owner(inter_owner, inter_owner + net.nInter());
+                for (int i = 0; i < net.nInter(); ++i)
+                    if (owner[i] < 0 || owner[i] >= world)
+                        return fail("intersection " + std::to_string(i) + " is given rank " + std::to_string(owner[i]) +
+                                    ", outside [0, " + std::to_string(world) + ")");
+                g->part = cfb::Partition::fromOwners(net, owner, world);
+            } else {
+                g->part = cfb::Partition::columnStrips(net, world);
+            }
+        }
+        std::string err = e->h.configureShard(r, g->part);
+        if (!err.empty()) return fail(err);
     }
     {   // same process: the "peer mappings" are the arenas themselves
         const char *tr = getenv("CITYFLOW_B200_SHARD_TRANSPORT");
@@ -2089,6 +2109,15 @@ cfb_shard_group *cfb_shard_group_create(const char *config_file, int world, int 
         };
     }
     return g.release();
+}
+
+cfb_shard_group *cfb_shard_group_create(const char *config_file, int world, int device) {
+    return shardGroupCreate(config_file, world, device, nullptr);
+}
+
+cfb_shard_group *cfb_debug_shard_group_create_cut(const char *config_file, int world, int device, const int32_t *inter_owner) {
+    if (!inter_owner) { g_createError = "sharded engine: no intersection owners given"; return nullptr; }
+    return shardGroupCreate(config_file, world, device, inter_owner);
 }
 
 void cfb_shard_group_destroy(cfb_shard_group *g) {
@@ -2154,7 +2183,7 @@ int cfb_shard_group_counters(cfb_shard_group *g, int64_t out[2]) {
 int cfb_shard_group_lane_counts(cfb_shard_group *g, int32_t *out, int n, int waiting) {
     const int nL = g->ranks[0]->h.net.nLanes();
     if (n < nL) return CFB_ERR_ARGUMENT;
-    cfb::Partition part = cfb::Partition::columnStrips(g->ranks[0]->h.net, (int) g->ranks.size());
+    const cfb::Partition &part = g->part;
     std::vector<int32_t> tmp(nL);
     for (size_t r = 0; r < g->ranks.size(); ++r) {
         if (waiting) g->ranks[r]->h.dev->laneWaitingVehicleCount(tmp.data()); else g->ranks[r]->h.dev->laneVehicleCount(tmp.data());
@@ -2165,7 +2194,7 @@ int cfb_shard_group_lane_counts(cfb_shard_group *g, int32_t *out, int n, int wai
 
 // every running vehicle of the owning ranks (same record as cfb_debug_vehicles)
 int64_t cfb_shard_group_debug_vehicles(cfb_shard_group *g, void *out, int64_t cap) {
-    cfb::Partition part = cfb::Partition::columnStrips(g->ranks[0]->h.net, (int) g->ranks.size());
+    const cfb::Partition &part = g->part;
     struct Rec { int32_t w[8]; double d[3]; int64_t e; };
     int64_t total = 0;
     std::vector<Rec> tmp;

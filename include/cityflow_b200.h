@@ -180,6 +180,10 @@ int cfb_shard_group_lane_counts(cfb_shard_group *g, int32_t *out, int n, int wai
 int64_t cfb_shard_group_debug_vehicles(cfb_shard_group *g, void *out, int64_t cap);
 /* sums over the group's ranks: out = {cfb_vehicle_steps, cfb_tie_count} */
 int cfb_shard_group_counters(cfb_shard_group *g, int64_t out[2]);
+/* Test support: a loop-back group cut by `inter_owner` (the rank of every intersection, virtual ones
+ * included, in roadnet order) instead of column strips.  A lane belongs to the rank of its END
+ * intersection.  Returns null, with the reason in cfb_last_error, if the cut is refused. */
+cfb_shard_group *cfb_debug_shard_group_create_cut(const char *config_file, int world, int device, const int32_t *inter_owner);
 
 /* Test support: full dynamic state of every running vehicle, drivable-major in list order.
  * Record = 8 x int32 {flow, index, priority, drivable, leader flow, leader index, blocker flow,

@@ -245,7 +245,7 @@ def short_hops(seed: int, rows: int = 4, cols: int = 5):
 MERGE_GROUPS = {"P": (0, 0, 1, 1), "Q": (0, 0, 0), "R": (1, 1, 1, 1)}   # target lane on I -> J of every approach road
 
 
-def merge_ties(seed: int):
+def merge_ties(seed: int, groups=MERGE_GROUPS, background=True):
     """(roadnet, flows): single-lane approach roads into one merge intersection I, then a two-lane road I -> J to a
     second real intersection J and an exit road.  The approach roads are parallel translates of each other along y
     (lane lengths are then computed from x alone, so they are bit-equal), and so are their laneLinks into I -> J:
@@ -256,12 +256,14 @@ def merge_ties(seed: int):
     flow per approach road: its vehicles run in lockstep and enter their target lane in the same step at the same
     distance.  P sends a pair into each lane (equal distances on neighbouring lanes), Q three and R four vehicles into
     one lane.  Two background flows with their own parameters use approaches of their own, one per target lane, so
-    that ties also land behind survivors."""
+    that ties also land behind survivors.  `groups` / `background` replace the merge groups and drop the background
+    flows (merge_16)."""
     rng = random.Random(seed)
     w_i, w_j = rng.uniform(10, 14), rng.uniform(8, 12)
     d_ij, l_app, l_exit = rng.uniform(220, 260), 300.0, 300.0
-    approaches = [("%s%d" % (g, k), t) for g, lanes in sorted(MERGE_GROUPS.items()) for k, t in enumerate(lanes)]
-    approaches += [("B0", 0), ("B1", 1)]
+    approaches = [("%s%d" % (g, k), t) for g, lanes in sorted(groups.items()) for k, t in enumerate(lanes)]
+    if background:
+        approaches += [("B0", 0), ("B1", 1)]
     inters = {"I": {"id": "n_I", "point": {"x": 0.0, "y": 0.0}, "width": w_i, "roads": [], "roadLinks": [], "virtual": False},
               "J": {"id": "n_J", "point": {"x": d_ij, "y": 0.0}, "width": w_j, "roads": [], "roadLinks": [], "virtual": False},
               "X": {"id": "n_X", "point": {"x": d_ij + l_exit, "y": 0.0}, "width": 0, "roads": [], "roadLinks": [], "virtual": True}}
@@ -292,13 +294,13 @@ def merge_ties(seed: int):
     net = {"intersections": [inters[k] for k in sorted(inters)], "roads": roads}
     flows = []
     timing = {"P": (12.0, 0), "Q": (16.0, 4), "R": (20.0, 8)}
-    for g in sorted(MERGE_GROUPS):
+    for g in sorted(groups):
         veh = _vehicle(rng, rng.uniform(4.0, 5.0), rng.uniform(2.0, 2.5), rng.uniform(11.0, 13.0), rng.uniform(1.0, 1.5))
-        interval, start = timing[g]
-        for k in range(len(MERGE_GROUPS[g])):
+        interval, start = timing.get(g, (20.0, 0))
+        for k in range(len(groups[g])):
             flows.append({"vehicle": dict(veh), "route": ["r_%s%d__I" % (g, k), "r_I__J", "r_J__X"], "interval": interval,
                           "startTime": start, "endTime": -1})
-    for name in ("B0", "B1"):
+    for name in ("B0", "B1") if background else ():
         flows.append({"vehicle": _vehicle(rng, rng.uniform(4.0, 6.0), rng.uniform(2.0, 2.5), rng.uniform(10.0, 14.0), rng.uniform(1.0, 1.5)),
                       "route": ["r_%s__I" % name, "r_I__J", "r_J__X"], "interval": rng.uniform(15.0, 25.0), "startTime": rng.choice([0, 2]),
                       "endTime": -1})
@@ -317,7 +319,10 @@ def merge_approach_lanes(cfg: str) -> dict:
     return out
 
 
-SHAPES = {"long_queue": (long_queue, 1.0), "star": (star, 1.0), "short_hops": (short_hops, 2.0), "merge_ties": (merge_ties, 1.0)}
+# merge_16: sixteen approaches in lockstep into lane 0 of I -> J -- ENT_CAP = 16 entrants of one lane in one step, one
+# full mover message when I -> J is a seam lane.  No background flows: a 17th entrant would overflow ENT_CAP.
+SHAPES = {"long_queue": (long_queue, 1.0), "star": (star, 1.0), "short_hops": (short_hops, 2.0), "merge_ties": (merge_ties, 1.0),
+          "merge_16": (lambda seed: merge_ties(seed, {"W": (0,) * 16}, background=False), 1.0)}
 
 
 def write(shape: str, directory: str, seed: int = 1, lane_change: bool = False) -> str:
@@ -413,3 +418,205 @@ class Reach:
     def __str__(self):
         return "max vehicles on a lane %d, on a laneLink %d; max entrants into one drivable in one step %d; max drivables " \
                "crossed in one step %d" % (self.lane_occ, self.link_occ, self.entrants, self.hops)
+
+
+# ---------------------------------------------------------------- cuts of a sharded run and what a run reached at them
+def partition(cfg: str, world: int, owners=None) -> dict:
+    """The product's partition of `cfg` (tests/partition_probe.cpp, built into oracle/_build like loader_tables): column
+    strips, or Partition::fromOwners of `owners` (one rank per intersection, virtual ones included).  Keys: inter_owner,
+    inter_virtual, lane_owner, lane_feeder, lane_start, lane_end, boundary[a][b] (lanes fed by a, owned by b)."""
+    import json
+    import os
+    import subprocess
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    probe = os.path.join(root, "oracle", "_build", "partition_probe")
+    csrc = os.path.join(root, "cityflow_b200", "csrc")
+    srcs = [os.path.join(root, "tests", "partition_probe.cpp"), os.path.join(csrc, "partition.cpp"), os.path.join(csrc, "roadnet.cpp")]
+    os.makedirs(os.path.dirname(probe), exist_ok=True)
+    deps = srcs + [os.path.join(csrc, "partition.h"), os.path.join(csrc, "roadnet.h")]
+    if not os.path.exists(probe) or os.path.getmtime(probe) < max(os.path.getmtime(f) for f in deps):
+        subprocess.check_call(["g++", "-std=c++17", "-O1"] + srcs + ["-o", probe])
+    args = [probe, cfg, str(world)]
+    if owners is not None:
+        args += ["-1", ",".join(str(int(o)) for o in owners)]
+    return json.loads(subprocess.check_output(args))
+
+
+def look_ahead(cfg: str) -> float:
+    """How far beyond its lane end a vehicle of `cfg` may look (HostEngine::configureShard's formula over the flows'
+    vehicles): Partition::validate refuses a seam lane no longer than this."""
+    import json
+    c = json.load(open(cfg))
+    look = 0.0
+    for f in json.load(open(c["dir"] + c["flowFile"])):
+        v = f["vehicle"]
+        look = max(look, v["maxSpeed"] * v["maxSpeed"] / v["usualNegAcc"] / 2 + v["maxSpeed"] * c["interval"] * 2)
+    return look
+
+
+def scattered_owners(cfg: str, world: int, seed: int) -> list:
+    """A seeded random rank for every intersection, with both ends of every road that has a lane no longer than the
+    look-ahead put on one rank (so that Partition::validate accepts the cut), and every rank given at least one real
+    intersection where the network has enough of them."""
+    p, static = partition(cfg, 1), loader_tables(cfg)
+    length = [float.fromhex(x) for x in static["lane_length"]]
+    look = look_ahead(cfg)
+    rng = random.Random(seed)
+    n = len(p["inter_owner"])
+    real = [i for i in range(n) if not p["inter_virtual"][i]]
+    own = [rng.randrange(world) for _ in range(n)]
+    for k, i in enumerate(rng.sample(real, min(world, len(real)))):
+        own[i] = k
+    root = list(range(n))
+
+    def find(i):
+        while root[i] != i:
+            root[i] = root[root[i]]
+            i = root[i]
+        return i
+    for l in range(p["n_lanes"]):
+        if length[l] <= look:
+            a, b = find(p["lane_start"][l]), find(p["lane_end"][l])
+            root[max(a, b)] = min(a, b)
+    return [own[find(i)] for i in range(n)]
+
+
+def checkerboard_owners(cfg: str, world: int = 2) -> list:
+    """Rank (column + row) % world of every intersection, columns and rows counted over the distinct x and y of the
+    intersections' points: on a grid, every road is a seam road and every rank has seams in all four directions."""
+    import json
+    c = json.load(open(cfg))
+    pts = [(i["point"]["x"], i["point"]["y"]) for i in json.load(open(c["dir"] + c["roadnetFile"]))["intersections"]]
+    xs, ys = sorted({x for x, _ in pts}), sorted({y for _, y in pts})
+    return [(xs.index(x) + ys.index(y)) % world for x, y in pts]
+
+
+class SeamReach:
+    """What a sharded run reached at its seams, fed the restatement's state (VEH_DTYPE records) after every step:
+
+    * ``crossed``: vehicles entering a seam lane, per direction (feeder, owner) -> (total, most in one step);
+    * ``max_movers``: the most vehicles entering one seam lane in one step (one mover message, ENT_CAP = 16 records);
+    * ``max_queue``: the longest queue on a seam lane, as the share of the lane's length from its end back to the last
+      of the halted (speed < 0.1) vehicles that follow its head without a moving one between them, and ``halted_feeding``: the most halted vehicles on laneLinks into a seam
+      lane whose queue covered 90 % of it (they wait on the ghost tail);
+    * ``spawns`` / ``finishes``: vehicles appearing on / leaving the network from a seam lane, ``virtual_spawns``: those
+      spawns onto a seam lane fed by a virtual intersection;
+    * ``max_blk_sent``: the most blocker changes one rank sends in one step (a changed blocker of a vehicle on one of
+      its drivables, or one of its vehicles leaving the network), and ``foreign_blockers``: vehicle steps whose blocker
+      is on a drivable of another rank (a chain that leaves the rank);
+    * from the cut alone: ``neighbours`` per rank, ``virtual_fed`` seam lanes (their feeder is a virtual intersection),
+      ``empty_ranks`` (ranks without a real intersection) and the seam lanes each rank feeds and owns."""
+
+    def __init__(self, static, part):
+        self.n_lanes = static["n_lanes"]
+        self.length = [float.fromhex(x) for x in static["lane_length"]]
+        self.link_end = static["link_end"]
+        lane_owner = part["lane_owner"]
+        link_owner = [0] * len(self.link_end)
+        for l, links in enumerate(static["lane_out"]):
+            for k in links:
+                link_owner[k] = lane_owner[l]          # a laneLink sits in the intersection its start lane ends at
+        self.owner = np.array(list(lane_owner) + link_owner)
+        W = part["world"]
+        self.world = W
+        self.seam = {l: (a, b) for a in range(W) for b in range(W) for l in part["boundary"][a][b]}
+        self.neighbours = [sum(1 for q in range(W) if q != r and part["boundary"][r][q] + part["boundary"][q][r]) for r in range(W)]
+        self.feeds = [sum(len(part["boundary"][r][q]) for q in range(W)) for r in range(W)]
+        self.owns = [sum(len(part["boundary"][q][r]) for q in range(W)) for r in range(W)]
+        virt = part["inter_virtual"]
+        self.virtual_lanes = {l for l in self.seam if virt[part["lane_start"][l]]}
+        self.virtual_fed = len(self.virtual_lanes)
+        has_real = {o for o, v in zip(part["inter_owner"], virt) if not v}
+        self.empty_ranks = [r for r in range(W) if r not in has_real]
+        self.crossed = {}
+        self.max_movers = self.spawns = self.virtual_spawns = self.finishes = self.max_blk_sent = self.foreign_blockers = self.halted_feeding = 0
+        self.max_queue = 0.0
+        self.prev = {}
+
+    def add(self, vehicles):
+        nl = self.n_lanes
+        now = {(int(f), int(c)): (int(d), (int(bf), int(bc))) for f, c, d, bf, bc in
+               zip(vehicles["flow"], vehicles["cnt"], vehicles["drivable"], vehicles["blocker_flow"], vehicles["blocker_cnt"])}
+        into, pairs, sent = {}, {}, [0] * self.world
+        for key, (d, blk) in now.items():
+            p = self.prev.get(key)
+            if p is None:
+                self.spawns += d in self.seam
+                self.virtual_spawns += d in self.virtual_lanes
+            elif p[0] != d and d in self.seam:
+                into[d] = into.get(d, 0) + 1
+                pairs[self.seam[d]] = pairs.get(self.seam[d], 0) + 1
+            if p is not None and p[1] != blk:
+                sent[self.owner[d]] += 1
+            if blk[0] >= 0 or blk[1] >= 0:
+                b = now.get(blk)
+                self.foreign_blockers += b is not None and self.owner[b[0]] != self.owner[d]
+        for key, (d, _) in self.prev.items():
+            if key not in now:
+                self.finishes += d in self.seam
+                sent[self.owner[d]] += 1
+        self.max_movers = max([self.max_movers] + list(into.values()))
+        self.max_blk_sent = max([self.max_blk_sent] + sent)
+        for pr, n in pairs.items():
+            tot, most = self.crossed.get(pr, (0, 0))
+            self.crossed[pr] = (tot + n, max(most, n))
+        drv, dis, spd = vehicles["drivable"], vehicles["dis"], vehicles["speed"]
+        halted = spd < 0.1
+        full = set()
+        for l in set(int(x) for x in drv[halted]) & set(self.seam):
+            on = np.nonzero(drv == l)[0]
+            on = on[np.argsort(-dis[on], kind="stable")]
+            run = np.cumprod(halted[on])                 # the halted vehicles from the head back, up to the first moving one
+            if run[0]:
+                q = (self.length[l] - float(dis[on[int(run.sum()) - 1]])) / self.length[l]
+                self.max_queue = max(self.max_queue, q)
+                if q >= 0.9:
+                    full.add(l)
+        if full:
+            on_links = drv[halted & (drv >= nl)]
+            self.halted_feeding = max(self.halted_feeding, int(sum(self.link_end[d - nl] in full for d in on_links)))
+        self.prev = now
+
+    def __str__(self):
+        crossed = ", ".join("%d->%d %d (%d in one step)" % (a, b, t, m) for (a, b), (t, m) in sorted(self.crossed.items()))
+        return ("seam lanes fed / owned per rank %s / %s, neighbours per rank %s, %d seam lanes fed by a virtual intersection, "
+                "ranks without a real intersection %s; crossings %s; at most %d movers into one seam lane in one step; "
+                "longest halted queue on a seam lane %.3f of its length, %d halted vehicles on laneLinks into a full one; "
+                "%d spawns onto seam lanes (%d onto virtual-fed ones), %d finishes on seam lanes; at most %d blocker changes sent by one rank in one step, "
+                "%d vehicle steps blocked across ranks" %
+                (self.feeds, self.owns, self.neighbours, self.virtual_fed, self.empty_ranks, crossed or "none", self.max_movers,
+                 self.max_queue, self.halted_feeding, self.spawns, self.virtual_spawns, self.finishes, self.max_blk_sent, self.foreign_blockers))
+
+
+def group_vs_restatement(grp, cfg, steps, reach=None, check=lambda s: True):
+    """Step a loop-back group (cityflow_b200.capi.CShardGroup, or its emulated-device form) and the restatement together.
+    At every step `check(s)` accepts: vehicle count, lane and waiting counts, the ranks' summed counters (vehicle steps,
+    ties), and every running vehicle -- every field, and the order of every drivable's list (the group lists each rank's
+    vehicles drivable by drivable in list order) -- must be equal.  `reach` (SeamReach) is fed every step.  Returns the
+    restatement."""
+    from oracle import harness as H
+    ora = H.PortOracle(cfg)
+    vehicle_steps = 0
+    for s in range(1, steps + 1):
+        grp.next_step()
+        ora.next_step()
+        st = ora.snapshot(with_order=check(s))
+        vehicle_steps += st.vehicle_count
+        if reach is not None:
+            reach.add(st.vehicles)
+        if not check(s):
+            continue
+        assert grp.vehicle_count() == st.vehicle_count, "step %d" % s
+        assert grp.counters() == (vehicle_steps, ora.tie_count()), "counters, step %d" % s
+        assert np.array_equal(grp.lane_counts(ora.n_lanes), st.lane_count), "lane counts, step %d" % s
+        assert np.array_equal(grp.lane_counts(ora.n_lanes, True), st.lane_waiting), "waiting counts, step %d" % s
+        mine = grp.debug_vehicles()
+        a, b = np.sort(mine, order=["flow", "cnt"]), np.sort(st.vehicles, order=["flow", "cnt"])
+        assert len(a) == len(b), "step %d" % s
+        for f in ("flow", "cnt", "priority", "drivable", "dis", "speed", "leader_flow", "leader_cnt", "blocker_flow",
+                  "blocker_cnt", "gap", "enter_ll_time"):
+            assert np.array_equal(a[f], b[f]), "step %d field %s" % (s, f)
+        listed = mine[np.argsort(mine["drivable"], kind="stable")]
+        want = np.concatenate([o for o in st.order if len(o)] or [np.zeros((0, 2), np.int32)])
+        assert np.array_equal(np.stack([listed["flow"], listed["cnt"]], 1), want), "list order, step %d" % s
+    return ora
