@@ -20,6 +20,30 @@ VEH_DTYPE = np.dtype([
 REF_DTYPE = np.dtype([("flow", "<i4"), ("index", "<i4")])
 REPLAY_DTYPE = np.dtype([("drivable", "<i4"), ("distance", "<f8"), ("flow", "<i4"), ("index", "<i4"),
                          ("length", "<f8"), ("width", "<f8")], align=True)   # cfb_replay_vehicle
+REPLAY_LC_DTYPE = np.dtype([("v", REPLAY_DTYPE), ("shadow_depth", "<i4"), ("lane_change_dir", "<i4"),
+                            ("offset", "<f8")], align=True)                     # cfb_replay_vehicle_lc
+REF_SHADOW_SHIFT = 24          # CFB_REF_SHADOW_SHIFT: bits 24-30 of cfb_vehicle_ref.index count "_shadow" suffixes
+REF_INDEX_MASK = 0x00ffffff    # CFB_REF_INDEX_MASK
+
+
+def vehicle_name(flow: int, index: int) -> str:
+    """The reference's id of a cfb_vehicle_ref (include/cityflow_b200.h)."""
+    base = "manually_pushed_%d" % (index & REF_INDEX_MASK) if flow == -2 else "flow_%d_%d" % (flow, index & REF_INDEX_MASK)
+    return base + "_shadow" * (index >> REF_SHADOW_SHIFT)
+
+
+def parse_vehicle_name(name: str):
+    """(flow, index) of a reference id, shadow suffixes in index's bits 24-30; None if it names no vehicle."""
+    depth = 0
+    while name.endswith("_shadow") and depth < 127:
+        name, depth = name[:-7], depth + 1
+    m = re.fullmatch(r"flow_(\d+)_(\d+)|manually_pushed_(\d+)", name)
+    if not m:
+        return None
+    flow, index = (int(m.group(1)), int(m.group(2))) if m.group(3) is None else (-2, int(m.group(3)))
+    if index > REF_INDEX_MASK:
+        return None
+    return flow, index | (depth << REF_SHADOW_SHIFT)
 
 
 def declared_symbols() -> list:
@@ -80,6 +104,7 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_replay_destroy": (None, [vp]),
         "cfb_replay_roadnet_json": (i64, [vp, vp, i64]),
         "cfb_replay_format_step": (i64, [vp, vp, i64, vp, vp, i64]),
+        "cfb_replay_format_step_lc": (i64, [vp, vp, i64, vp, vp, i64]),
         "cfb_push_vehicle": (i32, [vp, vp, vp, i32]),
         "cfb_snapshot": (vp, [vp]),
         "cfb_archive_destroy": (None, [vp]),
@@ -365,4 +390,13 @@ class CReplay:
         n = int(self.lib.cfb_replay_format_step(self.h, v.ctypes.data, len(v), ph.ctypes.data, None, 0))
         buf = ctypes.create_string_buffer(n)
         self.lib.cfb_replay_format_step(self.h, v.ctypes.data, len(v), ph.ctypes.data, buf, n)
+        return buf.value.decode()
+
+    def format_step_lc(self, vehicles: np.ndarray, phases: np.ndarray) -> str:
+        """format_step with lane change (cfb_replay_format_step_lc): REPLAY_LC_DTYPE records."""
+        v = np.ascontiguousarray(vehicles, REPLAY_LC_DTYPE)
+        ph = np.ascontiguousarray(phases, np.int32)
+        n = int(self.lib.cfb_replay_format_step_lc(self.h, v.ctypes.data, len(v), ph.ctypes.data, None, 0))
+        buf = ctypes.create_string_buffer(n)
+        self.lib.cfb_replay_format_step_lc(self.h, v.ctypes.data, len(v), ph.ctypes.data, buf, n)
         return buf.value.decode()

@@ -108,6 +108,8 @@ public:
     std::ofstream logOut;                                    // Engine::logOut engine.h:40
     std::vector<SpeedRec> replayRecs;
     std::vector<ReplayVehicle> replayVeh;
+    std::vector<DeviceSim::LcDebugRec> replayRecsLc;
+    std::vector<ReplayVehicleLc> replayVehLc;
     std::vector<int32_t> replayPhase;
     std::string replayLine;
     std::mt19937 rnd;
@@ -654,6 +656,7 @@ public:
     // after this step, one line.  Gathers from the device (synchronises), so stepping with
     // saveReplay on is as slow as it is in the reference.
     void writeReplayLine() {
+        if (laneChange) { writeReplayLineLc(); return; }
         const int n = dev->runningVehicles(replayRecs);
         std::sort(replayRecs.begin(), replayRecs.end(), [this](const SpeedRec &a, const SpeedRec &b) {
             return slots[a.slot].priority < slots[b.slot].priority;   // vehiclePool order (engine.cpp:780-790)
@@ -669,6 +672,28 @@ public:
         replay->formatStep(replayVeh.data(), (size_t) n, replayPhase.data(), replayLine);
         logOut << replayLine << std::endl;
     }
+    // the same with lane change: real vehicles only (getRunningVehicles, engine.cpp:780-790), drawn off the lane centre
+    // while they change lanes, with their last change direction.  The offsets and directions come with the lane-change
+    // records of every running vehicle (one copy of the device state per step, like the rest of a replay step).
+    void writeReplayLineLc() {
+        drain();   // take-overs: a shadow that became the vehicle is written under its parent's id
+        dev->debugDumpLc(replayRecsLc);
+        std::sort(replayRecsLc.begin(), replayRecsLc.end(), [this](const DeviceSim::LcDebugRec &a, const DeviceSim::LcDebugRec &b) {
+            return slots[a.slot].priority < slots[b.slot].priority;
+        });
+        replayVehLc.clear();
+        for (const DeviceSim::LcDebugRec &r : replayRecsLc) {
+            if (r.partnerType == 2) continue;   // a shadow still changing is not real (vehicle.h:278)
+            const SlotInfo &s = slots[r.slot];
+            const VehicleTemplate &t = templates[s.tmplId];
+            replayVehLc.push_back(ReplayVehicleLc{ReplayVehicle{r.drivable, r.dis, s.flow, s.index, t.len, t.width}, s.shadow ? 1 : 0,
+                                                  r.lastDir, r.offset});
+        }
+        replayPhase.resize(net.nInter());
+        dev->phases(replayPhase.data());
+        replay->formatStepLc(replayVehLc.data(), replayVehLc.size(), replayPhase.data(), replayLine);
+        logOut << replayLine << std::endl;
+    }
     void finishStep() {
         h2dBytes += (long long) batch.size() * sizeof(SpawnRec) + sizeof(int);
         finishedDirty = true;
@@ -682,6 +707,9 @@ public:
         std::vector<int32_t> spare(256);
         for (auto &x : spare) { x = allocSlot(); slots[x].live = false; }
         prepareStep();                                   // (ensures device capacity for every slot handed out so far)
+        for (const SpawnRec &r : batch)                  // the id's counter must leave room for the shadow suffixes
+            if (slots[r.slot].index > CFB_REF_INDEX_MASK)
+                throw std::runtime_error("vehicle counter beyond 2^24 - 1: a lane-change engine cannot name " + vehicleName(slots[r.slot]));
         std::vector<DeviceSim::LcShadow> created;
         dev->stepLcBegin(batch.data(), (int) batch.size(), spare.data(), (int) spare.size(), created);
         std::vector<int32_t> prio(created.size());
@@ -799,11 +827,13 @@ public:
         if (resetRnd) rnd.seed(seed);
     }
 
+    // Engine::vehicleMap: a shadow still changing is found under its own id (engine.cpp:815), and once the change is
+    // complete under its parent's (engine.cpp:238-239) -- the id refOf() reports for it then.  Call after drain().
     int slotOfId(int flow, int index) {
         if (!idMapValid) {
             idToSlot.clear();
             for (size_t s = 0; s < slots.size(); ++s)
-                if (slots[s].live) idToSlot[key(slots[s].flow, slots[s].index)] = (int) s;
+                if (slots[s].live) idToSlot[key(slots[s].flow, refOf((int) s).index)] = (int) s;
             idMapValid = true;
         }
         auto it = idToSlot.find(key(flow, index));
@@ -1148,7 +1178,11 @@ public:
         hs.templates = templates;
     }
 
-    cfb_vehicle_ref refOf(int slot) const { return cfb_vehicle_ref{slots[slot].flow, slots[slot].index}; }
+    // The reference's id (cfb_vehicle_ref): a shadow still changing lanes is "<parent's id>_shadow"; when the change
+    // completes it takes its parent's id (lanechange.cpp:120-121), so drain() must have seen the take-over.
+    cfb_vehicle_ref refOf(int slot) const {
+        return cfb_vehicle_ref{slots[slot].flow, slots[slot].index | (slots[slot].shadow ? 1 << CFB_REF_SHADOW_SHIFT : 0)};
+    }
 };
 
 }  // namespace cfb
@@ -1320,6 +1354,12 @@ int64_t cfb_get_vehicle_speed(cfb_engine *e, cfb_vehicle_ref *ids, double *speed
     CFB_TRY(e,
         cfb::HostEngine &h = e->h;
         int n = h.dev->runningVehicles(e->recs);
+        if (h.laneChange) {   // Engine::getRunningVehicles skips shadows still changing (isReal, engine.cpp:785)
+            h.drain();
+            e->recs.erase(std::remove_if(e->recs.begin(), e->recs.end(), [&h](const cfb::SpeedRec &r) { return h.slots[r.slot].shadow; }),
+                          e->recs.end());
+            n = (int) e->recs.size();
+        }
         // vehiclePool order = ascending priority (engine.cpp:780-790)
         std::sort(e->recs.begin(), e->recs.end(), [&h](const cfb::SpeedRec &a, const cfb::SpeedRec &b) {
             return h.slots[a.slot].priority < h.slots[b.slot].priority;
@@ -1341,6 +1381,7 @@ int64_t cfb_get_vehicles(cfb_engine *e, int include_waiting, cfb_vehicle_ref *id
         h.drain();
         int64_t n = 0;
         for (auto &kv : h.pool.sorted()) {
+            if (h.slots[kv.second].shadow) continue;   // not real (engine.cpp:785)
             if (n < cap && ids) ids[n] = h.refOf(kv.second);
             ++n;
         }
@@ -1352,6 +1393,7 @@ int64_t cfb_get_lane_vehicles(cfb_engine *e, int64_t *lane_begin, int n_lanes_pl
     if (n_lanes_plus1 < e->h.net.nLanes() + 1) { e->lastError = "output buffer too small"; return CFB_ERR_ARGUMENT; }
     CFB_TRY(e,
         std::vector<int32_t> slots; std::vector<int32_t> beg;
+        if (e->h.laneChange) e->h.drain();   // names after take-overs
         e->h.dev->laneVehicleSlots(slots, beg);
         for (size_t l = 0; l < beg.size(); ++l) lane_begin[l] = beg[l];
         for (size_t i = 0; i < slots.size() && (int64_t) i < cap; ++i) ids[i] = e->h.refOf(slots[i]);
@@ -1364,8 +1406,9 @@ int cfb_get_leader(cfb_engine *e, cfb_vehicle_ref v, cfb_vehicle_ref *leader, in
         cfb::HostEngine &h = e->h;
         h.cancelAhead();
         h.drain();
-        const int vs = h.slotOfId(v.flow, v.index);
+        int vs = h.slotOfId(v.flow, v.index);
         if (vs < 0) throw std::runtime_error("Vehicle not found");
+        if (h.slots[vs].shadow) vs = h.slotOfId(v.flow, v.index & CFB_REF_INDEX_MASK);   // its partner's leader (engine.cpp:841-844)
         int ls = h.dev->leaderSlotOf(vs);
         *found = ls >= 0;
         if (ls >= 0) *leader = h.refOf(ls);
@@ -1457,6 +1500,12 @@ int64_t cfb_replay_roadnet_json(cfb_replay *r, char *out, int64_t cap) { return 
 int64_t cfb_replay_format_step(cfb_replay *r, const cfb_replay_vehicle *v, int64_t n, const int32_t *phase, char *out, int64_t cap) {
     static_assert(sizeof(cfb_replay_vehicle) == sizeof(cfb::ReplayVehicle), "cfb_replay_vehicle layout");
     r->w->formatStep(reinterpret_cast<const cfb::ReplayVehicle *>(v), (size_t) n, phase, r->buf);
+    return copyOut(r->buf, out, cap);
+}
+
+int64_t cfb_replay_format_step_lc(cfb_replay *r, const cfb_replay_vehicle_lc *v, int64_t n, const int32_t *phase, char *out, int64_t cap) {
+    static_assert(sizeof(cfb_replay_vehicle_lc) == sizeof(cfb::ReplayVehicleLc), "cfb_replay_vehicle_lc layout");
+    r->w->formatStepLc(reinterpret_cast<const cfb::ReplayVehicleLc *>(v), (size_t) n, phase, r->buf);
     return copyOut(r->buf, out, cap);
 }
 
@@ -1703,7 +1752,8 @@ extern "C" int64_t cfb_get_vehicle_info(cfb_engine *e, cfb_vehicle_ref v, char *
             if (rid >= 0) {
                 const auto &pb = h.routing->planBeg();
                 int plan = (int) (std::upper_bound(pb.begin(), pb.end(), st.planIdx) - pb.begin()) - 1;
-                const int rpos = (st.planIdx - pb[plan]) / 2;
+                // a shadow's lane plan (lane change) starts at a road inside its route
+                const int rpos = (h.laneChange ? h.routing->planRoadPos(plan) : 0) + (st.planIdx - pb[plan]) / 2;
                 const auto &roads = h.routing->route(rid).roads;
                 for (size_t k = rpos; k < roads.size(); ++k) route += n.roadId[roads[k]] + " ";
             }

@@ -22,25 +22,42 @@ using namespace py::literals;
 
 namespace {
 
+// "_shadow" once per shadow level (bits 24-30 of index, include/cityflow_b200.h)
 std::string vehicleName(const cfb_vehicle_ref &r) {
-    if (r.flow == -2) return "manually_pushed_" + std::to_string(r.index);
-    return "flow_" + std::to_string(r.flow) + "_" + std::to_string(r.index);
+    const int32_t index = r.index & CFB_REF_INDEX_MASK;
+    std::string id = r.flow == -2 ? "manually_pushed_" + std::to_string(index)
+                                  : "flow_" + std::to_string(r.flow) + "_" + std::to_string(index);
+    for (int k = r.index >> CFB_REF_SHADOW_SHIFT; k > 0; --k) id += "_shadow";
+    return id;
 }
 
 bool parseVehicleName(const std::string &id, cfb_vehicle_ref &out) {
+    static const std::string suffix = "_shadow";
+    size_t end = id.size();
+    int depth = 0;
+    while (end > suffix.size() && id.compare(end - suffix.size(), suffix.size(), suffix) == 0 && depth < 127) {
+        end -= suffix.size();
+        ++depth;
+    }
+    const std::string base = id.substr(0, end);
     try {
-        if (id.compare(0, 16, "manually_pushed_") == 0) {
+        bool manual = base.compare(0, 16, "manually_pushed_") == 0;
+        if (manual) {
             out.flow = -2;
-            out.index = std::stoi(id.substr(16));
-            return true;
-        }
-        if (id.compare(0, 5, "flow_") == 0) {
-            size_t us = id.find('_', 5);
+            out.index = std::stoi(base.substr(16));
+        } else if (base.compare(0, 5, "flow_") == 0) {
+            size_t us = base.find('_', 5);
             if (us == std::string::npos) return false;
-            out.flow = std::stoi(id.substr(5, us - 5));
-            out.index = std::stoi(id.substr(us + 1));
-            return vehicleName(out) == id;
+            out.flow = std::stoi(base.substr(5, us - 5));
+            out.index = std::stoi(base.substr(us + 1));
+        } else {
+            return false;
         }
+        if (depth > 0) {
+            if (out.index < 0 || out.index > CFB_REF_INDEX_MASK) return false;
+            out.index |= depth << CFB_REF_SHADOW_SHIFT;
+        }
+        return manual || vehicleName(out) == id;
     } catch (...) {
     }
     return false;

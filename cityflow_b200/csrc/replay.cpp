@@ -158,21 +158,22 @@ std::string ReplayWriter::roadnetJson() const {
     return s;
 }
 
-void ReplayWriter::formatStep(const ReplayVehicle *v, size_t n, const int *phase, std::string &out) const {
-    out.clear();
-    for (size_t k = 0; k < n; ++k) {
-        const std::vector<Pt> &pts = drvPoints_[v[k].drivable];
-        const Pt pos = pointAt(pts, v[k].dis);           // Vehicle::getPoint with offset 0 (vehicle.cpp:82-84)
-        const Pt dir = directionAt(pts, v[k].dis);
-        put(out, pos.x); out.push_back(' ');
-        put(out, pos.y); out.push_back(' ');
-        put(out, std::atan2(dir.y, dir.x)); out.push_back(' ');
-        if (v[k].flow == -2) out += "manually_pushed_" + std::to_string(v[k].index);
-        else out += "flow_" + std::to_string(v[k].flow) + "_" + std::to_string(v[k].index);
-        out += " 0 ";                                    // lastLaneChangeDirection: 0 without lane change
-        put(out, v[k].len); out.push_back(' ');
-        put(out, v[k].width); out.push_back(',');
-    }
+void ReplayWriter::putVehicle(std::string &out, const ReplayVehicle &v, Pt pos, int shadowDepth, int dir) const {
+    const Pt d = directionAt(drvPoints_[v.drivable], v.dis);
+    put(out, pos.x); out.push_back(' ');
+    put(out, pos.y); out.push_back(' ');
+    put(out, std::atan2(d.y, d.x)); out.push_back(' ');
+    if (v.flow == -2) out += "manually_pushed_" + std::to_string(v.index);
+    else out += "flow_" + std::to_string(v.flow) + "_" + std::to_string(v.index);
+    for (int k = 0; k < shadowDepth; ++k) out += "_shadow";
+    out.push_back(' ');
+    out += std::to_string(dir);
+    out.push_back(' ');
+    put(out, v.len); out.push_back(' ');
+    put(out, v.width); out.push_back(',');
+}
+
+void ReplayWriter::putLights(std::string &out, const int *phase) const {
     out.push_back(';');
     for (int r = 0; r < net_.nRoads(); ++r) {
         const int in = net_.roadEndInter[r];
@@ -191,6 +192,31 @@ void ReplayWriter::formatStep(const ReplayVehicle *v, size_t n, const int *phase
         }
         out.push_back(',');
     }
+}
+
+void ReplayWriter::formatStep(const ReplayVehicle *v, size_t n, const int *phase, std::string &out) const {
+    out.clear();
+    for (size_t k = 0; k < n; ++k)   // Vehicle::getPoint with offset 0 (vehicle.cpp:82-84); lastLaneChangeDirection 0
+        putVehicle(out, v[k], pointAt(drvPoints_[v[k].drivable], v[k].dis), 0, 0);
+    putLights(out, phase);
+}
+
+void ReplayWriter::formatStepLc(const ReplayVehicleLc *v, size_t n, const int *phase, std::string &out) const {
+    constexpr double eps = 1e-8;   // utility.h:15
+    out.clear();
+    for (size_t k = 0; k < n; ++k) {
+        const ReplayVehicle &u = v[k].v;
+        const double off = v[k].offset;
+        Pt pos = pointAt(drvPoints_[u.drivable], u.dis);
+        if (!(std::fabs(off) < eps) && u.drivable < net_.nLanes()) {   // Vehicle::getPoint vehicle.cpp:81-105
+            const int next = off > 0 ? u.drivable + 1 : u.drivable - 1;   // lanes of a road are consecutive, by index
+            const Pt q = pointAt(drvPoints_[next], u.dis);
+            const double pct = (off > 0 ? 2 * off : -2 * off) / (net_.laneWidth[u.drivable] + net_.laneWidth[next]);
+            pos = Pt{q.x * pct + pos.x * (1 - pct), q.y * pct + pos.y * (1 - pct)};
+        }
+        putVehicle(out, u, pos, v[k].shadowDepth, v[k].dir);
+    }
+    putLights(out, phase);
 }
 
 }  // namespace cfb

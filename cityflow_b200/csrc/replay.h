@@ -28,6 +28,13 @@ struct ReplayVehicle {
     double len, width;   // VehicleInfo len / width
 };
 
+struct ReplayVehicleLc { // a running vehicle of a lane-change run (cfb_replay_vehicle_lc)
+    ReplayVehicle v;
+    int shadowDepth;     // "_shadow" suffixes of the id
+    int dir;             // LaneChange::lastDir
+    double offset;       // LaneChangeInfo::offset
+};
+
 // JSON output pieces (json_write.cpp).  putJsonNumber: the shortest digit string that parses back to `v`, laid out like
 // the reference's printer ("2.0", "12.34", "1.234e33").  putJsonNumberLikeRapidjson: the digits rapidjson's writer
 // (Grisu2) emits -- the archive writer uses it so that the reference reads back the doubles it would from its own file.
@@ -43,10 +50,14 @@ public:
     // one replayLogFile line (no trailing newline).  vehicles: running vehicles in ascending
     // priority; phase[i]: current phase index of intersection i (ignored for virtual ones).
     void formatStep(const ReplayVehicle *vehicles, size_t n, const int *phase, std::string &out) const;
+    // the same with lane change: off-centre positions, suffixed ids, change directions
+    void formatStepLc(const ReplayVehicleLc *vehicles, size_t n, const int *phase, std::string &out) const;
     // Intersection::getOutline roadnet.cpp:750-817 (flattened x0,y0,x1,y1,...)
     std::vector<double> outline(int intersection) const;
 
 private:
+    void putVehicle(std::string &out, const ReplayVehicle &v, Pt pos, int shadowDepth, int dir) const;
+    void putLights(std::string &out, const int *phase) const;
     const RoadNet &net_;
     std::vector<std::vector<Pt>> drvPoints_;      // lanes then laneLinks
     std::vector<double> roadWidth_;

@@ -26,11 +26,20 @@ extern "C" {
 typedef struct cfb_engine cfb_engine;
 
 /* A vehicle as the reference names it: "flow_<flow>_<index>" (flow.cpp:11) or, for vehicles
- * added with push_vehicle, "manually_pushed_<index>" (engine.cpp:714; flow == -2). */
+ * added with push_vehicle, "manually_pushed_<index>" (engine.cpp:714; flow == -2).
+ *
+ * With "laneChange": true a car that changes lanes gets a shadow in the target lane, named
+ * "<car's id>_shadow" (engine.cpp:814).  While the change runs both are listed; when it completes the
+ * car leaves and the shadow carries on under the car's own id (lanechange.cpp:120-121, engine.cpp:238-239),
+ * so a name never holds more than one suffix.  `index` carries the number of "_shadow" suffixes in its
+ * bits 24-30 (CFB_REF_SHADOW_SHIFT) and the counter in bits 0-23 (CFB_REF_INDEX_MASK): a lane-change
+ * engine refuses to create a vehicle whose counter does not fit.  Without laneChange bits 24-30 are 0. */
 typedef struct cfb_vehicle_ref {
     int32_t flow;
     int32_t index;
 } cfb_vehicle_ref;
+#define CFB_REF_SHADOW_SHIFT 24
+#define CFB_REF_INDEX_MASK 0x00ffffff
 
 enum {
     CFB_OK = 0,
@@ -264,6 +273,18 @@ int64_t cfb_replay_roadnet_json(cfb_replay *r, char *out, int64_t cap);
  * per intersection (cfb_num_intersections() entries) */
 int64_t cfb_replay_format_step(cfb_replay *r, const cfb_replay_vehicle *vehicles, int64_t n, const int32_t *phase,
                                char *out, int64_t cap);
+/* The same with lane change: the position is moved off the lane centre towards the neighbour lane by
+ * `offset` (Vehicle::getPoint vehicle.cpp:81-105), the id gets `shadow_depth` "_shadow" suffixes and the
+ * line carries `lane_change_dir` (LaneChange::lastDir, lanechange.cpp:130-135) instead of 0.  `v.index`
+ * holds the counter alone. */
+typedef struct {
+    cfb_replay_vehicle v;
+    int32_t shadow_depth;
+    int32_t lane_change_dir;   /* -1 inner, 1 outer, 0 none */
+    double offset;             /* LaneChangeInfo::offset, > 0 towards the lane of the next higher index */
+} cfb_replay_vehicle_lc;
+int64_t cfb_replay_format_step_lc(cfb_replay *r, const cfb_replay_vehicle_lc *vehicles, int64_t n, const int32_t *phase,
+                                  char *out, int64_t cap);
 
 #ifdef __cplusplus
 }
