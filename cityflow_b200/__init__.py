@@ -82,6 +82,84 @@ def lane_observation_tensors(engine, stream=None):
     return o.lane_ids, o.vehicle_count, o.waiting_count, o.speed_sum
 
 
+class VehicleObservations:
+    """Zero-copy table of every running vehicle as torch CUDA tensors, for a policy on the engine's GPU.
+
+    Rows are drivable-major: lanes in ``engine.lane_ids()`` order, then the laneLinks (``drivable_ids``
+    holds the ids of both); the rows of drivable ``d`` are ``drivable_begin[d]:drivable_begin[d + 1]``, in
+    list order, front first -- for a lane the order ``get_lane_vehicles()`` reports.  Columns: ``slot``,
+    ``priority`` and ``drivable`` (int32), ``distance`` and ``speed`` (float64, bit-equal to
+    ``get_vehicle_distance()`` / ``get_vehicle_speed()``), ``shadow`` (uint8, 1 for a lane-change shadow).
+    ``count`` (int32, one element) is the number of rows in use (= ``get_vehicle_count()``); the rows from
+    ``count`` to the tensors' length are padding with ``slot == -1``, so a policy of fixed shape can mask them.
+    Waiting vehicles are not rows.
+
+    ``(slot, priority)`` is a row's vehicle handle: :func:`set_vehicle_speeds_tensor` takes it, and
+    ``vehicle_ids(slots)`` turns slots into the reference's ids.  ``refresh()`` re-computes the table on the
+    engine's stream, ordered against ``stream`` (default: torch's current stream on that device) in both
+    directions, without a host copy or wait; the tensors alias the engine's buffers and keep their storage
+    across refreshes.  ``clone()`` what must survive the next refresh.  Single-GPU engines only.
+    """
+
+    _COLUMNS = (("slot", "<i4"), ("priority", "<i4"), ("drivable", "<i4"), ("distance", "<f8"), ("speed", "<f8"),
+                ("shadow", "|u1"))
+
+    def __init__(self, engine, stream=None):
+        self.engine = engine
+        self._device = engine.device()
+        self._ptrs = None
+        self.drivable_ids = engine.drivable_ids()
+        self.refresh(stream)
+
+    def _stream(self, stream):
+        if stream is None:
+            import torch
+            return torch.cuda.current_stream(self._device).cuda_stream
+        return int(getattr(stream, "cuda_stream", stream))
+
+    def refresh(self, stream=None):
+        o = self.engine.observe_vehicles_device(self._stream(stream))
+        ptrs = tuple(o[k] for k, _ in self._COLUMNS) + (o["drivable_begin"], o["count"], o["capacity"])
+        if ptrs != self._ptrs:   # first call, or the engine re-allocated its buffers
+            import torch
+            dev = torch.device("cuda", o["device"])
+            mk = lambda ptr, n, ts: torch.as_tensor(_DeviceArray(self.engine, ptr, n, ts), device=dev)  # noqa: E731
+            for k, ts in self._COLUMNS:
+                setattr(self, k, mk(o[k], o["capacity"], ts))
+            self.drivable_begin = mk(o["drivable_begin"], o["n_drivables"] + 1, "<i4")
+            self.count = mk(o["count"], 1, "<i4")
+            self._ptrs = ptrs
+        return self
+
+    def vehicle_ids(self, slots):
+        """The reference's ids of the vehicles in ``slots`` (a tensor, array or list; host side: it waits for the
+        device), ``None`` where a slot holds no vehicle.  A shadow still changing lanes is ``"<id>_shadow"``."""
+        if hasattr(slots, "tolist"):
+            slots = slots.tolist()
+        return self.engine.vehicle_ids([int(s) for s in slots])
+
+
+def set_vehicle_speeds_tensor(engine, slot, priority, speed, stream=None):
+    """``set_vehicle_speed`` for many vehicles at once from torch CUDA tensors (no host copy, no host wait).
+
+    ``slot`` / ``priority`` (int32) and ``speed`` (float64): contiguous, the same length, on the engine's GPU,
+    produced on ``stream`` (default: torch's current stream there).  Entry ``i`` sets a one-shot custom speed
+    for the coming step on the vehicle whose :class:`VehicleObservations` handle is ``(slot[i], priority[i])``;
+    entries with ``slot < 0`` are skipped, so the padded columns of a table can be passed as they are.  A handle
+    that no longer names a running vehicle, or a slot given twice, raises ``RuntimeError`` at the engine's next
+    synchronising call (``get_vehicle_count()``, the getters).  Single-GPU engines only.
+    """
+    import torch
+    n = slot.numel()
+    for t, dt in ((slot, torch.int32), (priority, torch.int32), (speed, torch.float64)):
+        if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.device.index == engine.device() and t.numel() == n):
+            raise ValueError("slot / priority must be contiguous int32 and speed contiguous float64 CUDA tensors of one "
+                             "length on the engine's device")
+    if stream is None:
+        stream = torch.cuda.current_stream(engine.device()).cuda_stream
+    engine.set_vehicle_speeds_device(slot.data_ptr(), priority.data_ptr(), speed.data_ptr(), n, int(stream))
+
+
 def set_tl_phases_tensor(engine, phases, stream=None):
     """``set_tl_phase`` for every traffic light at once from a torch CUDA tensor (no host copy).
 

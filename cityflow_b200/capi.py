@@ -120,6 +120,10 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_debug_step_grids": (i32, [vp, vp]),
         "cfb_shard_group_counters": (i32, [vp, vp]),
         "cfb_debug_shard_group_create_cut": (vp, [cp, i32, i32, vp]),
+        "cfb_observe_vehicles_device": (i32, [vp, vp, vp]),
+        "cfb_set_vehicle_speeds_device": (i32, [vp, vp, vp, vp, i64, vp]),
+        "cfb_vehicle_refs": (i32, [vp, vp, i64, vp]),
+        "cfb_drivable_id": (cp, [vp, i64]),
     }
     for name, (res, args) in sig.items():
         if not hasattr(lib, name):
@@ -128,6 +132,14 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         fn.restype = res
         fn.argtypes = args
     return lib
+
+
+class DeviceVehicleObs(ctypes.Structure):
+    """cfb_device_vehicle_obs: device pointers of the per-vehicle observation table (include/cityflow_b200.h)."""
+    _fields_ = [("slot", ctypes.c_void_p), ("priority", ctypes.c_void_p), ("drivable", ctypes.c_void_p),
+                ("distance", ctypes.c_void_p), ("speed", ctypes.c_void_p), ("shadow", ctypes.c_void_p),
+                ("drivable_begin", ctypes.c_void_p), ("count", ctypes.c_void_p), ("capacity", ctypes.c_int64),
+                ("n_drivables", ctypes.c_int32), ("device", ctypes.c_int32)]
 
 
 class CEngine:
@@ -284,6 +296,26 @@ class CEngine:
         h2d, d2h = ctypes.c_int64(0), ctypes.c_int64(0)
         self._check(self.lib.cfb_transfer_bytes(self.h, ctypes.byref(h2d), ctypes.byref(d2h)))
         return h2d.value, d2h.value
+
+    def observe_vehicles_device(self, stream: int = 0) -> DeviceVehicleObs:
+        """Refresh the per-vehicle observation table (cfb_observe_vehicles_device) and return its pointers."""
+        o = DeviceVehicleObs()
+        self._check(self.lib.cfb_observe_vehicles_device(self.h, stream, ctypes.byref(o)))
+        return o
+
+    def set_vehicle_speeds_device(self, slot: int, priority: int, speed: int, n: int, stream: int = 0):
+        """cfb_set_vehicle_speeds_device: slot / priority / speed are device addresses of n entries each."""
+        self._check(self.lib.cfb_set_vehicle_speeds_device(self.h, slot, priority, speed, n, stream))
+
+    def vehicle_refs(self, slots):
+        """cfb_vehicle_refs: REF_DTYPE record per slot, (-1, -1) where the slot holds no vehicle."""
+        s = np.ascontiguousarray(slots, np.int32)
+        out = np.zeros(len(s), REF_DTYPE)
+        self._check(self.lib.cfb_vehicle_refs(self.h, s.ctypes.data, len(s), out.ctypes.data))
+        return out
+
+    def drivable_ids(self):
+        return [self.lib.cfb_drivable_id(self.h, d).decode() for d in range(self.n_drivables)]
 
     def snapshot(self) -> "CArchive":
         a = self.lib.cfb_snapshot(self.h)

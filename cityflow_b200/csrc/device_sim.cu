@@ -191,6 +191,17 @@ __global__ void __launch_bounds__(256) k_gather_running(View V, SpeedRec *out, i
     }
 }
 
+}  // namespace cfb
+#include "device_vehobs.cuh"
+namespace cfb {
+// The per-vehicle table (device_vehobs.cuh): tile sums, then offsets + bucket copies.  And the batched custom speed.
+__global__ void __launch_bounds__(VOBS_TILE) k_vobs_sums(View V, VehObsTable T) { vobsTileSums(V, T, blockIdx.x); }
+__global__ void __launch_bounds__(VOBS_TILE) k_vobs_fill(View V, VehObsTable T) { vobsFill(V, T, blockIdx.x, gridDim.x); }
+__global__ void __launch_bounds__(256) k_vspeed(View V, const int *slot, const int *priority, const double *speed, int n,
+                                                int *stamp, int slotCap, int call) {
+    vspeedApply(V, slot, priority, speed, n, stamp, slotCap, call, blockIdx.x, gridDim.x);
+}
+
 __global__ void k_lane_slots(View V, int *out, const int *laneBeg) {
     const int d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -369,6 +380,16 @@ struct DeviceSim::Impl {
     cudaEvent_t obsReady = nullptr, obsConsumed = nullptr;
     cudaEvent_t actReady = nullptr, actTaken = nullptr;   // setPhasesFromDevice()
     bool hPhaseStale = false;          // the device copy is newer than hPhase (phases were set on the device)
+    DevBuf<int> vobsI;                 // observeVehicles(): slot | priority | drivable (capacity rows each), drivable begin,
+                                       //   count, previous count, tile sums
+    DevBuf<double> vobsD;              //                    distance | speed
+    DevBuf<unsigned char> vobsShadow;
+    VehObsTable vobs{};
+    int vobsTiles = 0;
+    cudaEvent_t vobsReady = nullptr, vobsConsumed = nullptr;
+    DevBuf<int> speedStamp;            // setCustomSpeedsFromDevice(): per slot, the last call that named it
+    int speedCall = 0;
+    cudaEvent_t speedReady = nullptr, speedTaken = nullptr;
     std::vector<cudaEvent_t> stepEv;   // timed-step brackets (bench)
     size_t stepEvUsed = 0;
     DevBuf<unsigned char> flushBuf;
@@ -1262,6 +1283,88 @@ DeviceObs DeviceSim::observeOnDevice(void *consumerStream) {
     o.nLanes = nL;
     o.device = I.opt.device;
     return o;
+}
+
+DeviceVehObs DeviceSim::observeVehicles(void *consumerStream) {
+    Impl &I = *impl_;
+    if (I.V.owned) throw std::runtime_error("observeVehicles: not available on one rank of a sharded run");
+    const size_t cap = (size_t) std::max(I.P, 1), nD = (size_t) I.V.nDrv;
+    const int tiles = (int) std::max<size_t>(1, (nD + VOBS_TILE - 1) / VOBS_TILE);
+    const size_t nI = 3 * cap + (nD + 1) + 2 + (size_t) tiles;
+    if (I.vobsI.n < nI) {   // first call (the row capacity is the position capacity, fixed when the engine is made)
+        I.vobsI.alloc(nI);
+        I.vobsD.alloc(2 * cap);
+        I.vobsShadow.alloc(cap);
+        CFB_CUDA(cudaMemsetAsync(I.vobsI.p, 0xff, cap * sizeof(int), I.stream));                       // slot: all padding
+        CFB_CUDA(cudaMemsetAsync(I.vobsI.p + cap, 0, (nI - cap) * sizeof(int), I.stream));             // count 0
+        CFB_CUDA(cudaMemsetAsync(I.vobsD.p, 0, 2 * cap * sizeof(double), I.stream));
+        CFB_CUDA(cudaMemsetAsync(I.vobsShadow.p, 0, cap, I.stream));
+        VehObsTable &T = I.vobs;
+        T.slot = I.vobsI.p; T.priority = T.slot + cap; T.drivable = T.priority + cap;
+        T.drvBegin = T.drivable + cap; T.count = T.drvBegin + nD + 1; T.prevCount = T.count + 1; T.tileSum = T.prevCount + 1;
+        T.distance = I.vobsD.p; T.speed = I.vobsD.p + cap; T.shadow = I.vobsShadow.p;
+        I.vobsTiles = tiles;
+        if (!I.vobsReady) {
+            CFB_CUDA(cudaEventCreateWithFlags(&I.vobsReady, cudaEventDisableTiming));
+            CFB_CUDA(cudaEventCreateWithFlags(&I.vobsConsumed, cudaEventDisableTiming));
+        }
+    }
+    cudaStream_t cs = (cudaStream_t) consumerStream;
+    CFB_CUDA(cudaEventRecord(I.vobsConsumed, cs));         // the consumer's earlier reads finish before the refresh ...
+    CFB_CUDA(cudaStreamWaitEvent(I.stream, I.vobsConsumed, 0));
+    k_vobs_sums<<<I.vobsTiles, VOBS_TILE, 0, I.stream>>>(I.V, I.vobs);
+    k_vobs_fill<<<I.vobsTiles, VOBS_TILE, 0, I.stream>>>(I.V, I.vobs);
+    CFB_CUDA(cudaGetLastError());
+    CFB_CUDA(cudaEventRecord(I.vobsReady, I.stream));      // ... and its later reads see it, the host waiting for neither
+    CFB_CUDA(cudaStreamWaitEvent(cs, I.vobsReady, 0));
+    launches_ += 2;
+    const VehObsTable &T = I.vobs;
+    DeviceVehObs o;
+    o.slot = T.slot; o.priority = T.priority; o.drivable = T.drivable;
+    o.distance = T.distance; o.speed = T.speed; o.shadow = T.shadow;
+    o.drivableBegin = T.drvBegin; o.count = T.count;
+    o.capacity = (long long) cap;
+    o.nDrv = I.V.nDrv;
+    o.device = I.opt.device;
+    return o;
+}
+
+void DeviceSim::setCustomSpeedsFromDevice(const int32_t *slot, const int32_t *priority, const double *speed, long long n,
+                                          void *producerStream) {
+    Impl &I = *impl_;
+    if (I.V.owned) throw std::runtime_error("setCustomSpeedsFromDevice: not available on one rank of a sharded run");
+    if (n < 0 || n > INT_MAX) throw std::runtime_error("setCustomSpeedsFromDevice: entry count out of range");
+    if (!I.speedReady) {
+        CFB_CUDA(cudaEventCreateWithFlags(&I.speedReady, cudaEventDisableTiming));
+        CFB_CUDA(cudaEventCreateWithFlags(&I.speedTaken, cudaEventDisableTiming));
+    }
+    if (I.speedStamp.n < (size_t) I.slotCap) {   // first call, or the slot table grew (ensureSlotCapacity synchronised)
+        I.speedStamp.alloc((size_t) I.slotCap);
+        CFB_CUDA(cudaMemsetAsync(I.speedStamp.p, 0, (size_t) I.slotCap * sizeof(int), I.stream));
+        I.speedCall = 0;
+    }
+    if (++I.speedCall == INT_MAX) {              // stamps of earlier calls must not match a later call's number
+        CFB_CUDA(cudaMemsetAsync(I.speedStamp.p, 0, (size_t) I.slotCap * sizeof(int), I.stream));
+        I.speedCall = 1;
+    }
+    cudaStream_t ps = (cudaStream_t) producerStream;
+    CFB_CUDA(cudaEventRecord(I.speedReady, ps));
+    CFB_CUDA(cudaStreamWaitEvent(I.stream, I.speedReady, 0));
+    if (n > 0) {
+        const int grid = (int) std::min<long long>((n + 255) / 256, (long long) I.numSMs * 8);
+        k_vspeed<<<grid, 256, 0, I.stream>>>(I.V, slot, priority, speed, (int) n, I.speedStamp.p, I.slotCap, I.speedCall);
+        CFB_CUDA(cudaGetLastError());
+        launches_ += 1;
+    }
+    CFB_CUDA(cudaEventRecord(I.speedTaken, I.stream));     // the producer may reuse its buffers after this
+    CFB_CUDA(cudaStreamWaitEvent(ps, I.speedTaken, 0));
+    I.mirrorStale = true;    // k_vspeed may raise ERR_VEHICLE_* outside a step
+}
+
+DeviceVehObs observeVehiclesOf(DeviceSim &dev, void *consumerStream) { return dev.observeVehicles(consumerStream); }
+void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot, const int32_t *priority, const double *speed, long long n,
+                       void *producerStream) {
+    dev.setCustomSpeedsFromDevice(slot, priority, speed, n, producerStream);
 }
 
 int DeviceSim::runningVehicles(std::vector<SpeedRec> &out) {

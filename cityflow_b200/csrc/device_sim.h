@@ -75,6 +75,8 @@ enum DeviceError : int {
     ERR_FINISHED_OVERFLOW = 16,
     ERR_PHASE_RANGE = 32,       // a phase index handed over on the device is outside the intersection's phase list
     ERR_SHARD_TIMEOUT = 64,     // sharded run: a peer's seam message did not arrive (peer crashed or stopped stepping)
+    ERR_VEHICLE_STALE = 128,    // a custom speed handed over on the device names a vehicle that is no longer running
+    ERR_VEHICLE_DUPLICATE = 256,   // ... or names one vehicle twice in one call
 };
 
 struct DeviceSimOptions {
@@ -103,6 +105,19 @@ struct DeviceObs {
     const int32_t *laneWaiting = nullptr;   // nLanes ints, speed < 0.1
     const double *laneSpeedSum = nullptr;   // nLanes doubles
     int nLanes = 0;
+    int device = 0;
+};
+
+// The per-vehicle observation table (device_vehobs.cuh): every running vehicle, drivable-major, list order.  Rows at and
+// beyond *count are padding (slot -1).
+struct DeviceVehObs {
+    const int32_t *slot = nullptr, *priority = nullptr, *drivable = nullptr;
+    const double *distance = nullptr, *speed = nullptr;
+    const uint8_t *shadow = nullptr;
+    const int32_t *drivableBegin = nullptr;   // nDrv + 1 entries
+    const int32_t *count = nullptr;           // device scalar
+    long long capacity = 0;                   // rows
+    int nDrv = 0;
     int device = 0;
 };
 
@@ -162,6 +177,14 @@ public:
     // (trafficlight.cpp:39-41); an out-of-range index leaves that light unchanged and raises
     // ERR_PHASE_RANGE.  No host synchronisation.
     void setPhasesFromDevice(const int32_t *phases, void *producerStream);
+    // The table of every running vehicle, refreshed on the engine's stream with the same handshake as observeOnDevice.
+    // The buffers are made once (their capacity is numPositions() rows); valid until the next call.
+    DeviceVehObs observeVehicles(void *consumerStream);
+    // setCustomSpeed for n vehicles at once, handed over on the device (produced on `producerStream`) as the handles of
+    // observation rows: entries with slot < 0 are skipped, a handle that no longer names the running vehicle raises
+    // ERR_VEHICLE_STALE, a slot named twice ERR_VEHICLE_DUPLICATE.  No host synchronisation.
+    void setCustomSpeedsFromDevice(const int32_t *slot, const int32_t *priority, const double *speed, long long n,
+                                   void *producerStream);
     // Observations (synchronise the stream).
     int vehicleCount();
     int errorFlags();
@@ -242,5 +265,12 @@ private:
     long long steps_ = 0;
     long long launches_ = 0;
 };
+
+// DeviceSim::observeVehicles / setCustomSpeedsFromDevice as free functions, for the C-ABI (host_engine.cpp).  Weak: the
+// host engine is also linked against a DeviceSim without the per-vehicle device path (the emulated device of the CPU
+// suite), where they stay null and the C-ABI reports the entry points as unavailable.
+__attribute__((weak)) DeviceVehObs observeVehiclesOf(DeviceSim &dev, void *consumerStream);
+__attribute__((weak)) void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot, const int32_t *priority, const double *speed,
+                                             long long n, void *producerStream);
 
 }  // namespace cfb

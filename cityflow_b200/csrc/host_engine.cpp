@@ -271,6 +271,8 @@ public:
             if (err & ERR_FINISHED_OVERFLOW) m += " finished ring overflow;";
             if (err & ERR_SHARD_TIMEOUT) m += " a peer rank's seam message did not arrive within 4 s (every rank of a sharded run must step in lock step);";
             if (err & ERR_PHASE_RANGE) m += " a phase index set from the device is out of range (the reference throws from phases.at(), trafficlight.cpp:17);";
+            if (err & ERR_VEHICLE_STALE) m += " Vehicle not found: a custom speed set from the device names a vehicle that is no longer running;";
+            if (err & ERR_VEHICLE_DUPLICATE) m += " a custom speed set from the device names one vehicle twice in one call;";
             throw std::runtime_error(m);
         }
     }
@@ -1213,6 +1215,7 @@ struct cfb_engine {
     cfb::HostEngine h;
     std::string lastError;
     std::vector<cfb::SpeedRec> recs;
+    std::vector<std::string> drivableIds;   // cfb_drivable_id
     std::unique_ptr<cfb::ShardTransport> transport;   // sharded run: destroyed before the device (see cfb_engine_destroy)
 };
 
@@ -1348,6 +1351,58 @@ int cfb_observe_device(cfb_engine *e, void *consumer_stream, cfb_device_obs *out
         out->device = o.device;
     )
     return CFB_OK;
+}
+
+// (weak: a DeviceSim build without the per-vehicle device path -- the emulated device of the CPU suite -- leaves them null)
+static void needVehicleObs() {
+    if (!cfb::observeVehiclesOf || !cfb::setCustomSpeedsOf)
+        throw std::runtime_error("per-vehicle device observations / actions are not part of this DeviceSim build");
+}
+
+int cfb_observe_vehicles_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_obs *out) {
+    if (!out) { e->lastError = "null output"; return CFB_ERR_ARGUMENT; }
+    CFB_TRY(e,
+        needVehicleObs();
+        const cfb::DeviceVehObs o = cfb::observeVehiclesOf(*e->h.dev, consumer_stream);
+        out->slot = o.slot; out->priority = o.priority; out->drivable = o.drivable;
+        out->distance = o.distance; out->speed = o.speed; out->shadow = o.shadow;
+        out->drivable_begin = o.drivableBegin; out->count = o.count;
+        out->capacity = o.capacity;
+        out->n_drivables = o.nDrv;
+        out->device = o.device;
+    )
+    return CFB_OK;
+}
+
+int cfb_set_vehicle_speeds_device(cfb_engine *e, const int32_t *slot, const int32_t *priority, const double *speed, int64_t n,
+                                  void *producer_stream) {
+    if (n < 0) { e->lastError = "negative entry count"; return CFB_ERR_ARGUMENT; }
+    if (n > 0 && (!slot || !priority || !speed)) { e->lastError = "null slot / priority / speed array"; return CFB_ERR_ARGUMENT; }
+    CFB_TRY(e, needVehicleObs(); cfb::setCustomSpeedsOf(*e->h.dev, slot, priority, speed, (long long) n, producer_stream);)
+    return CFB_OK;
+}
+
+int cfb_vehicle_refs(cfb_engine *e, const int32_t *slots, int64_t n, cfb_vehicle_ref *out) {
+    if (n < 0 || (n > 0 && (!slots || !out))) { e->lastError = "bad slot / output array"; return CFB_ERR_ARGUMENT; }
+    CFB_TRY(e,
+        cfb::HostEngine &h = e->h;
+        h.cancelAhead();   // (slots handed to next step's vehicles are not vehicles yet)
+        h.drain();         // vehicles that left, names after lane-change take-overs
+        for (int64_t i = 0; i < n; ++i) {
+            const int32_t s = slots[i];
+            out[i] = (s >= 0 && (size_t) s < h.slots.size() && h.slots[s].live) ? h.refOf(s) : cfb_vehicle_ref{-1, -1};
+        }
+    )
+    return CFB_OK;
+}
+
+const char *cfb_drivable_id(cfb_engine *e, int64_t d) {
+    cfb::HostEngine &h = e->h;
+    const int64_t nD = (int64_t) h.net.nLanes() + h.net.nLinks();
+    if (d < 0 || d >= nD) return nullptr;
+    if (e->drivableIds.empty())
+        for (int64_t k = 0; k < nD; ++k) e->drivableIds.push_back(h.drivableName((int) k));
+    return e->drivableIds[d].c_str();
 }
 
 int64_t cfb_get_vehicle_speed(cfb_engine *e, cfb_vehicle_ref *ids, double *speed, double *distance, int64_t cap) {

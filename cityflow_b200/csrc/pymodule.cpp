@@ -159,6 +159,40 @@ public:
         d["device"] = py::int_(o.device);
         return d;
     }
+    // device pointers of the per-vehicle observation table, ordered against CUDA stream `stream`
+    py::dict observeVehiclesDevice(uintptr_t stream) {
+        cfb_device_vehicle_obs o{};
+        check(cfb_observe_vehicles_device(e_, (void *) stream, &o));
+        py::dict d;
+        d["slot"] = py::int_((uintptr_t) o.slot);
+        d["priority"] = py::int_((uintptr_t) o.priority);
+        d["drivable"] = py::int_((uintptr_t) o.drivable);
+        d["distance"] = py::int_((uintptr_t) o.distance);
+        d["speed"] = py::int_((uintptr_t) o.speed);
+        d["shadow"] = py::int_((uintptr_t) o.shadow);
+        d["drivable_begin"] = py::int_((uintptr_t) o.drivable_begin);
+        d["count"] = py::int_((uintptr_t) o.count);
+        d["capacity"] = py::int_(o.capacity);
+        d["n_drivables"] = py::int_(o.n_drivables);
+        d["device"] = py::int_(o.device);
+        return d;
+    }
+    // the reference's ids of vehicle slots (None: the slot holds no vehicle)
+    py::list vehicleIds(const std::vector<int32_t> &slots) {
+        std::vector<cfb_vehicle_ref> refs(slots.size());
+        check(cfb_vehicle_refs(e_, slots.data(), (int64_t) slots.size(), refs.data()));
+        py::list out;
+        for (const cfb_vehicle_ref &r : refs) {
+            if (r.flow == -1 && r.index == -1) out.append(py::none());
+            else out.append(py::str(vehicleName(r)));
+        }
+        return out;
+    }
+    std::vector<std::string> drivableIds() {
+        std::vector<std::string> ids((size_t) cfb_num_drivables(e_));
+        for (size_t d = 0; d < ids.size(); ++d) ids[d] = cfb_drivable_id(e_, (int64_t) d);
+        return ids;
+    }
     py::dict getLaneVehicleCount() { return laneDict(false); }
     py::dict getLaneWaitingVehicleCount() { return laneDict(true); }
 
@@ -376,6 +410,14 @@ PYBIND11_MODULE(_cityflow_b200, m) {
         }, "phases_ptr"_a, "stream"_a = 0)
         .def("device", [](Engine &e) { return cfb_device(e.raw()); })
         .def("observe_device", &Engine::observeDevice, "stream"_a = 0)
+        .def("observe_vehicles_device", &Engine::observeVehiclesDevice, "stream"_a = 0)
+        .def("set_vehicle_speeds_device", [](Engine &e, uintptr_t slot, uintptr_t priority, uintptr_t speed, int64_t n, uintptr_t stream) {
+            if (cfb_set_vehicle_speeds_device(e.raw(), (const int32_t *) slot, (const int32_t *) priority, (const double *) speed, n,
+                                              (void *) stream) < 0)
+                throw std::runtime_error(cfb_last_error(e.raw()));
+        }, "slot_ptr"_a, "priority_ptr"_a, "speed_ptr"_a, "n"_a, "stream"_a = 0)
+        .def("vehicle_ids", &Engine::vehicleIds, "slots"_a)
+        .def("drivable_ids", &Engine::drivableIds)
         .def("synchronize", &Engine::synchronize);
     py::class_<Archive>(m, "Archive")
         .def(py::init<Engine &>())

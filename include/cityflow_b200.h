@@ -100,6 +100,46 @@ typedef struct {
     int32_t device;                      /* CUDA device ordinal the pointers live on */
 } cfb_device_obs;
 int cfb_observe_device(cfb_engine *e, void *consumer_stream, cfb_device_obs *out);
+/* Per-vehicle observations left ON THE DEVICE: one table of every running vehicle (waiting vehicles are not rows),
+ * refreshed and ordered against `consumer_stream` exactly as cfb_observe_device.  Rows are drivable-major: the lanes
+ * 0..cfb_num_lanes()-1 first, then the laneLinks (cfb_drivable_id); the rows of drivable d are
+ * [drivable_begin[d], drivable_begin[d+1]), in list order, front first -- for a lane, the order
+ * cfb_get_lane_vehicles reports.  Lane-change shadows are rows too (shadow = 1), as in getLaneVehicles and
+ * getVehicleCount (engine.cpp:817); getVehicleSpeed / getVehicles leave them out.  `count` is a device scalar
+ * (= drivable_begin[n_drivables]); rows from count to capacity are padding with slot = -1, so a consumer of fixed
+ * shape (a captured CUDA graph) can mask them.  (slot, priority) is the row's vehicle handle: see
+ * cfb_set_vehicle_speeds_device and cfb_vehicle_refs.  The pointers stay valid for the engine's lifetime; their
+ * content is valid until the next call.  Single-GPU engines only. */
+typedef struct {
+    const int32_t *slot;             /* vehicle handle: slot ... */
+    const int32_t *priority;         /* ... and Vehicle::priority (vehicle.cpp:45) */
+    const int32_t *drivable;         /* lane index, or cfb_num_lanes() + laneLink index */
+    const double *distance;          /* Vehicle::getDistance, bit-equal to cfb_get_vehicle_speed's */
+    const double *speed;             /* Vehicle::getSpeed */
+    const uint8_t *shadow;           /* 1: a lane-change shadow (Vehicle::isReal() == false) */
+    const int32_t *drivable_begin;   /* n_drivables + 1 entries */
+    const int32_t *count;            /* one int32: rows in use */
+    int64_t capacity;                /* rows of every column */
+    int32_t n_drivables;
+    int32_t device;                  /* CUDA device ordinal the pointers live on */
+} cfb_device_vehicle_obs;
+int cfb_observe_vehicles_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_obs *out);
+/* Engine::setVehicleSpeed (engine.cpp:827-834) for n vehicles at once, with the actions already ON THE DEVICE: slot,
+ * priority (int32) and speed (double), n entries each in device memory, consumed on the engine's stream after the work
+ * enqueued on `producer_stream` so far (as cfb_set_tl_phases_device).  Entries with slot < 0 are skipped, so the padded
+ * columns of a cfb_observe_vehicles_device table can be passed as they are.  Same state as the same
+ * cfb_set_vehicle_speed calls one by one: a one-shot custom speed for the coming step.  A handle that no longer names
+ * a running vehicle (the reference: "Vehicle not found") and a slot given twice in one call are reported as device
+ * errors by the next synchronising call; the other entries of the call are applied.  Single-GPU engines only. */
+int cfb_set_vehicle_speeds_device(cfb_engine *e, const int32_t *slot, const int32_t *priority, const double *speed, int64_t n,
+                                  void *producer_stream);
+/* The reference's ids of n vehicle slots (host memory, e.g. a copy of an observation table's slot column): out[i] =
+ * the id of the vehicle in slots[i] now, with "_shadow" for a shadow still changing lanes and the parent's id once the
+ * change completed; {-1, -1} for a slot that holds no vehicle. */
+int cfb_vehicle_refs(cfb_engine *e, const int32_t *slots, int64_t n, cfb_vehicle_ref *out);
+/* id of drivable d: lane ids first (cfb_lane_id), then laneLinks as "<start lane>_TO_<end lane>" (roadnet.h:478);
+ * NULL when out of range */
+const char *cfb_drivable_id(cfb_engine *e, int64_t d);
 /* Engine::getVehicleSpeed  engine.cpp:662-668 / getVehicleDistance :670-676: running vehicles in
  * vehiclePool (priority) order.  Returns the number of running vehicles (may exceed cap; only
  * cap entries are written); any of the three output pointers may be NULL. */

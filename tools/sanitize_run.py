@@ -5,7 +5,7 @@
     compute-sanitizer --tool initcheck python tools/sanitize_run.py
 
 Small networks so the instrumented kernels finish in seconds: single engine (step kernels, spawn
-ring, observation kernels, archive, vehicle setters), rlTrafficLight engine (host and device phase
+ring, observation kernels, archive, vehicle setters, the per-vehicle table and batched custom speed), rlTrafficLight engine (host and device phase
 setting, device-resident observations), lane change (its per-road
 kernels run roads concurrently: racecheck is the interesting tool there) and a 2-rank loop-back shard group
 (pack/unpack/seal kernels).
@@ -48,6 +48,17 @@ def main():
     for _ in range(30):
         eng.next_step()
     print("engine ok, vehicles", n, eng.get_vehicle_count())
+
+    # per-vehicle table and batched custom speed (device_vehobs.cuh), padded columns passed as they are
+    if os.environ.get("SAN_NO_TORCH") != "1":
+        import torch
+        vo = cityflow_b200.VehicleObservations(eng)
+        for _ in range(20):
+            vo.refresh()
+            cityflow_b200.set_vehicle_speeds_tensor(eng, vo.slot, vo.priority, (vo.speed * 0.5).contiguous())
+            eng.next_step()
+        torch.cuda.synchronize()
+        print("vehicle table ok, rows", int(vo.count.item()), eng.get_vehicle_count())
 
     rl = cityflow.Engine(cfg_rl, thread_num=1)
     inters = rl.intersection_ids()
