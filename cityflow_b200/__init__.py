@@ -139,6 +139,66 @@ class VehicleObservations:
         return self.engine.vehicle_ids([int(s) for s in slots])
 
 
+class IntersectionObservations:
+    """Zero-copy traffic-light observations as torch CUDA tensors: every light's phase and every movement's queue and
+    pressure, for a signal controller on the engine's GPU (MaxPressure, PressLight).
+
+    A movement is a roadLink; ``road_links`` (``engine.road_links()``) names them in the order of the movement
+    columns: intersections in ``engine.intersection_ids()`` order, each one's ``"roadLinks"`` in file order.
+    ``in_lanes(r)`` / ``out_lanes(r)`` are the distinct start / end lanes of r's laneLinks, ``in_lanes(i)`` /
+    ``out_lanes(i)`` their union over intersection i; ``count`` / ``waiting`` are ``get_lane_vehicle_count()`` /
+    ``get_lane_waiting_vehicle_count()``.  Per intersection (``[n_intersections]``): ``phase`` (int32, the index
+    ``set_tl_phase`` takes, -1 for a virtual intersection), ``phase_remaining`` (float64, remainDuration as
+    ``Archive.dump("x.json")`` writes it), ``pressure`` (int32, count over in_lanes(i) minus over out_lanes(i)),
+    ``queue`` (int32, waiting over in_lanes(i)).  Per movement (``[n_road_links]``, int32): ``movement_in``,
+    ``movement_in_waiting``, ``movement_out``, ``movement_inside`` (vehicles on its laneLinks) and
+    ``movement_pressure`` (in - out).  ``phase_pressure`` (int32 ``[n_intersections, max_phases]``): the sum of
+    movement_pressure over the movements available in each phase, ``INT32_MIN`` past ``phase_count[i]``, so
+    ``phase_pressure.argmax(1).to(torch.int32)`` is the MaxPressure action for :func:`set_tl_phases_tensor`.
+    Static: ``movement_begin`` ``[n_intersections + 1]``, ``movement_intersection``, ``phase_count`` and
+    ``phase_movements`` (uint8 ``[n_intersections, max_phases, max_movements]``).
+
+    ``refresh()`` re-computes the dynamic columns on the engine's stream after every ``set_tl_phase`` made before it,
+    ordered against ``stream`` (default: torch's current stream on that device) in both directions, without a host
+    copy or wait; the tensors alias the engine's buffers and keep their storage across refreshes.  ``clone()`` what
+    must survive the next refresh.  Single-GPU engines only.
+    """
+
+    _FLAT = (("phase", "<i4", "n_intersections"), ("phase_remaining", "<f8", "n_intersections"),
+             ("pressure", "<i4", "n_intersections"), ("queue", "<i4", "n_intersections"),
+             ("movement_in", "<i4", "n_road_links"), ("movement_in_waiting", "<i4", "n_road_links"),
+             ("movement_out", "<i4", "n_road_links"), ("movement_inside", "<i4", "n_road_links"),
+             ("movement_pressure", "<i4", "n_road_links"), ("movement_intersection", "<i4", "n_road_links"),
+             ("phase_count", "<i4", "n_intersections"))
+
+    def __init__(self, engine, stream=None):
+        import torch
+        self.engine = engine
+        self._device = engine.device()
+        self.road_links = engine.road_links()
+        o = engine.observe_intersections_device(self._stream(stream))
+        dev = torch.device("cuda", o["device"])
+        mk = lambda k, n, ts: torch.as_tensor(_DeviceArray(engine, o[k], n, ts), device=dev)  # noqa: E731
+        for k, ts, n in self._FLAT:
+            setattr(self, k, mk(k, o[n], ts))
+        nI, mP, mM = o["n_intersections"], o["max_phases"], o["max_movements"]
+        self.movement_begin = mk("movement_begin", nI + 1, "<i4")
+        self.phase_pressure = mk("phase_pressure", nI * mP, "<i4").view(nI, mP)
+        self.phase_movements = mk("phase_movements", nI * mP * mM, "|u1").view(nI, mP, mM)
+        self._ptrs = tuple(o[k] for k in sorted(o))
+
+    def _stream(self, stream):
+        if stream is None:
+            import torch
+            return torch.cuda.current_stream(self._device).cuda_stream
+        return int(getattr(stream, "cuda_stream", stream))
+
+    def refresh(self, stream=None):
+        o = self.engine.observe_intersections_device(self._stream(stream))
+        assert tuple(o[k] for k in sorted(o)) == self._ptrs
+        return self
+
+
 def set_vehicle_speeds_tensor(engine, slot, priority, speed, stream=None):
     """``set_vehicle_speed`` for many vehicles at once from torch CUDA tensors (no host copy, no host wait).
 

@@ -124,6 +124,9 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_set_vehicle_speeds_device": (i32, [vp, vp, vp, vp, i64, vp]),
         "cfb_vehicle_refs": (i32, [vp, vp, i64, vp]),
         "cfb_drivable_id": (cp, [vp, i64]),
+        "cfb_observe_intersections_device": (i32, [vp, vp, vp]),
+        "cfb_num_road_links": (i32, [vp]),
+        "cfb_road_link_info": (i32, [vp, i32, vp]),
     }
     for name, (res, args) in sig.items():
         if not hasattr(lib, name):
@@ -140,6 +143,21 @@ class DeviceVehicleObs(ctypes.Structure):
                 ("distance", ctypes.c_void_p), ("speed", ctypes.c_void_p), ("shadow", ctypes.c_void_p),
                 ("drivable_begin", ctypes.c_void_p), ("count", ctypes.c_void_p), ("capacity", ctypes.c_int64),
                 ("n_drivables", ctypes.c_int32), ("device", ctypes.c_int32)]
+
+
+class DeviceIntersectionObs(ctypes.Structure):
+    """cfb_device_intersection_obs: device pointers of the intersection / movement observations (include/cityflow_b200.h)."""
+    _fields_ = [(k, ctypes.c_void_p) for k in (
+        "phase", "phase_remaining", "pressure", "queue", "movement_in", "movement_in_waiting", "movement_out",
+        "movement_inside", "movement_pressure", "phase_pressure", "movement_begin", "movement_intersection",
+        "phase_count", "phase_movements")] + \
+        [(k, ctypes.c_int32) for k in ("n_intersections", "n_road_links", "max_phases", "max_movements", "device")]
+
+
+class RoadLink(ctypes.Structure):
+    """cfb_road_link: one movement as the roadnet file lists it."""
+    _fields_ = [("intersection", ctypes.c_int32), ("index", ctypes.c_int32), ("type", ctypes.c_int32),
+                ("pad", ctypes.c_int32), ("start_road", ctypes.c_char_p), ("end_road", ctypes.c_char_p)]
 
 
 class CEngine:
@@ -306,6 +324,21 @@ class CEngine:
     def set_vehicle_speeds_device(self, slot: int, priority: int, speed: int, n: int, stream: int = 0):
         """cfb_set_vehicle_speeds_device: slot / priority / speed are device addresses of n entries each."""
         self._check(self.lib.cfb_set_vehicle_speeds_device(self.h, slot, priority, speed, n, stream))
+
+    def observe_intersections_device(self, stream: int = 0) -> DeviceIntersectionObs:
+        """Refresh the intersection observations (cfb_observe_intersections_device) and return their pointers."""
+        o = DeviceIntersectionObs()
+        self._check(self.lib.cfb_observe_intersections_device(self.h, stream, ctypes.byref(o)))
+        return o
+
+    def road_links(self):
+        """cfb_road_link_info of every movement: (intersection, index, type, start road, end road) tuples."""
+        out = []
+        for r in range(self.lib.cfb_num_road_links(self.h)):
+            x = RoadLink()
+            self._check(self.lib.cfb_road_link_info(self.h, r, ctypes.byref(x)))
+            out.append((x.intersection, x.index, x.type, x.start_road.decode(), x.end_road.decode()))
+        return out
 
     def vehicle_refs(self, slots):
         """cfb_vehicle_refs: REF_DTYPE record per slot, (-1, -1) where the slot holds no vehicle."""

@@ -6,6 +6,7 @@
 // Host code only.  Included after device_view.cuh, like device_image.cuh.
 #pragma once
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstddef>
 #include <vector>
@@ -146,6 +147,110 @@ inline DeviceLayout deviceLayout(const RoadNet &net, View &V, double spacing) {
     for (int d = 0; d < nD; ++d)
         for (int p = L.off[d]; p < L.off[d + 1]; ++p) L.posDrv[p] = d;
     return L;
+}
+
+// The static tables of the intersection observations (device_tlobs.cuh), from the layout's laneLink and phase tables
+// (laneLinks are numbered intersection by intersection, roadLink by roadLink, so a roadLink's laneLinks are contiguous).
+// The kernel's tables are packed into one int array; the rest are public columns of DeviceIntersectionObs.
+struct IntObsLayout {
+    std::vector<int> ints;   // tl | inBeg | inLane | outBeg | outLane | rlInBeg | rlInLane | rlOutBeg | rlOutLane | rlLinkBeg
+    size_t tl = 0, inBeg = 0, inLane = 0, outBeg = 0, outLane = 0, rlInBeg = 0, rlInLane = 0, rlOutBeg = 0, rlOutLane = 0,
+           rlLinkBeg = 0;
+    int nTl = 0;
+    int maxPhases = 1, maxMovements = 1;       // (at least 1: every column is non-empty)
+    std::vector<int> movementBegin;            // nInter + 1: the roadLinks of intersection i (= RoadNet::interRoadLinkBeg)
+    std::vector<int> movementIntersection;     // nRL
+    std::vector<int> phaseCount;               // nInter, 0 for a virtual intersection
+    std::vector<unsigned char> phaseMovements; // [nInter][maxPhases][maxMovements]: roadLink k of i available in phase p
+    template <class Tab> void point(Tab &T, const int *at) const {
+        T.nTl = nTl; T.maxPhases = maxPhases; T.tl = at + tl;
+        T.inBeg = at + inBeg; T.inLane = at + inLane; T.outBeg = at + outBeg; T.outLane = at + outLane;
+        T.rlInBeg = at + rlInBeg; T.rlInLane = at + rlInLane; T.rlOutBeg = at + rlOutBeg; T.rlOutLane = at + rlOutLane;
+        T.rlLinkBeg = at + rlLinkBeg;
+    }
+    // The output ints: phase | pressure | queue | movement in | in waiting | out | inside | pressure | phase pressure |
+    // lane scratch | movement begin | movement intersection | phase count.  As they stand before the first refresh:
+    // phase -1 (what a virtual intersection keeps), phase pressure INT_MIN (what padding keeps), the static columns.
+    size_t outInts(const View &V) const {
+        return (size_t) 3 * V.nInter + 5 * (size_t) V.nRL + (size_t) V.nInter * maxPhases + V.nLanes + V.nInter + 1 +
+               V.nRL + V.nInter;
+    }
+    std::vector<int> initialInts(const View &V) const {
+        std::vector<int> v(outInts(V), 0);
+        const size_t nI = V.nInter, nRL = V.nRL, pp = 3 * nI + 5 * nRL, st = pp + nI * maxPhases + V.nLanes;
+        std::fill(v.begin(), v.begin() + nI, -1);
+        std::fill(v.begin() + pp, v.begin() + pp + nI * maxPhases, INT_MIN);
+        std::copy(movementBegin.begin(), movementBegin.end(), v.begin() + st);
+        std::copy(movementIntersection.begin(), movementIntersection.end(), v.begin() + st + nI + 1);
+        std::copy(phaseCount.begin(), phaseCount.end(), v.begin() + st + nI + 1 + nRL);
+        return v;
+    }
+    // T's output columns and o's pointers, with initialInts() at `ints`, nInter doubles at `dbl` and phaseMovements at `mv`
+    template <class Tab> void pointOut(Tab &T, DeviceIntersectionObs &o, const View &V, int *ints, double *dbl,
+                                       unsigned char *mv) const {
+        const int nI = V.nInter, nRL = V.nRL;
+        T.phase = ints; T.pressure = ints + nI; T.queue = ints + 2 * nI;
+        T.mvIn = ints + 3 * nI; T.mvInWaiting = T.mvIn + nRL; T.mvOut = T.mvInWaiting + nRL; T.mvInside = T.mvOut + nRL;
+        T.mvPressure = T.mvInside + nRL;
+        T.phasePressure = T.mvPressure + nRL;
+        T.laneWait = T.phasePressure + (size_t) nI * maxPhases;
+        T.remaining = dbl;
+        o.phase = T.phase; o.phaseRemaining = T.remaining; o.pressure = T.pressure; o.queue = T.queue;
+        o.movementIn = T.mvIn; o.movementInWaiting = T.mvInWaiting; o.movementOut = T.mvOut; o.movementInside = T.mvInside;
+        o.movementPressure = T.mvPressure; o.phasePressure = T.phasePressure;
+        o.movementBegin = T.laneWait + V.nLanes;
+        o.movementIntersection = o.movementBegin + nI + 1;
+        o.phaseCount = o.movementIntersection + nRL;
+        o.phaseMovements = mv;
+        o.nInter = nI; o.nRL = nRL; o.maxPhases = maxPhases; o.maxMovements = maxMovements;
+    }
+};
+inline IntObsLayout intObsLayout(const DeviceLayout &L, const View &V) {
+    IntObsLayout X;
+    const int nI = V.nInter, nRL = V.nRL, nK = V.nLinks;
+    std::vector<int> tl, rlLinkBeg(nRL + 1, 0);
+    for (int k = 0; k < nK; ++k) rlLinkBeg[L.llRoadLink[k] + 1] += 1;
+    for (int r = 0; r < nRL; ++r) rlLinkBeg[r + 1] += rlLinkBeg[r];
+    // distinct lanes in first-seen order, as CSR over `n` groups of laneLinks
+    auto distinct = [&](int n, auto linksOf, const std::vector<int> &lane, std::vector<int> &beg, std::vector<int> &out) {
+        beg.assign(n + 1, 0);
+        for (int g = 0; g < n; ++g) {
+            const int k0 = linksOf(g), k1 = linksOf(g + 1);
+            for (int k = k0; k < k1; ++k)
+                if (std::find(out.begin() + beg[g], out.end(), lane[k]) == out.end()) out.push_back(lane[k]);
+            beg[g + 1] = (int) out.size();
+        }
+    };
+    auto interLinks = [&](int i) { return rlLinkBeg[L.interRLBeg[i]]; };
+    auto rlLinks = [&](int r) { return rlLinkBeg[r]; };
+    std::vector<int> inBeg, inLane, outBeg, outLane, rlInBeg, rlInLane, rlOutBeg, rlOutLane;
+    distinct(nI, interLinks, L.llStartLane, inBeg, inLane);
+    distinct(nI, interLinks, L.llEndLane, outBeg, outLane);
+    distinct(nRL, rlLinks, L.llStartLane, rlInBeg, rlInLane);
+    distinct(nRL, rlLinks, L.llEndLane, rlOutBeg, rlOutLane);
+    X.phaseCount.assign(nI, 0);
+    for (int i = 0; i < nI; ++i) {
+        if (L.interVirtual[i]) continue;
+        tl.push_back(i);
+        X.phaseCount[i] = L.interPhaseBeg[i + 1] - L.interPhaseBeg[i];
+        X.maxPhases = std::max(X.maxPhases, X.phaseCount[i]);
+        X.maxMovements = std::max(X.maxMovements, L.interRLBeg[i + 1] - L.interRLBeg[i]);
+    }
+    X.nTl = (int) tl.size();
+    X.movementBegin = L.interRLBeg;
+    X.movementIntersection.assign(L.rlInter.begin(), L.rlInter.begin() + nRL);
+    X.phaseMovements.assign((size_t) std::max(nI, 1) * X.maxPhases * X.maxMovements, 0);
+    for (int i = 0; i < nI; ++i)
+        for (int p = 0; p < X.phaseCount[i]; ++p)
+            for (int k = 0; k < L.interRLBeg[i + 1] - L.interRLBeg[i]; ++k)
+                X.phaseMovements[((size_t) i * X.maxPhases + p) * X.maxMovements + k] =
+                    L.phaseAvail[L.phaseAvailBeg[L.interPhaseBeg[i] + p] + k];
+    auto add = [&X](const std::vector<int> &v) { const size_t at = X.ints.size(); X.ints.insert(X.ints.end(), v.begin(), v.end()); return at; };
+    X.tl = add(tl);
+    X.inBeg = add(inBeg); X.inLane = add(inLane); X.outBeg = add(outBeg); X.outLane = add(outLane);
+    X.rlInBeg = add(rlInBeg); X.rlInLane = add(rlInLane); X.rlOutBeg = add(rlOutBeg); X.rlOutLane = add(rlOutLane);
+    X.rlLinkBeg = add(rlLinkBeg);
+    return X;
 }
 
 // View::planBeg / planData; grown whenever a route is interned.

@@ -131,7 +131,7 @@ __global__ void __launch_bounds__(256) k_lane_waiting(View V, int *out) {  // en
     if (d >= V.nLanes) return;
     const int n = V.count[d], base = V.off[d];
     int c = 0;
-    for (int k = lane; k < n; k += 32) c += V.kin[base + k].y < 0.1;
+    for (int k = lane; k < n; k += 32) c += isWaiting(V.kin[base + k].y);
     for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     if (lane == 0) out[d] = c;
 }
@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(256) k_lane_obs(View V, int *cnt, int *wait, d
     double s = 0.0;
     for (int k = lane; k < n; k += 32) {
         const double v = V.kin[base + k].y;
-        c += v < 0.1;
+        c += isWaiting(v);
         s += v;
     }
     for (int o = 16; o; o >>= 1) {
@@ -201,6 +201,12 @@ __global__ void __launch_bounds__(256) k_vspeed(View V, const int *slot, const i
                                                 int *stamp, int slotCap, int call) {
     vspeedApply(V, slot, priority, speed, n, stamp, slotCap, call, blockIdx.x, gridDim.x);
 }
+
+}  // namespace cfb
+#include "device_tlobs.cuh"
+namespace cfb {
+// The intersection observations (device_tlobs.cuh): one warp per signalised intersection.
+__global__ void __launch_bounds__(TOBS_WARPS * 32) k_tobs(View V, IntObsTable T) { tobsFill(V, T, blockIdx.x, gridDim.x); }
 
 __global__ void k_lane_slots(View V, int *out, const int *laneBeg) {
     const int d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -390,6 +396,17 @@ struct DeviceSim::Impl {
     DevBuf<int> speedStamp;            // setCustomSpeedsFromDevice(): per slot, the last call that named it
     int speedCall = 0;
     cudaEvent_t speedReady = nullptr, speedTaken = nullptr;
+    DevBuf<int> tobsStatic;            // observeIntersections(): the kernel's tables (IntObsLayout::ints)
+    DevBuf<int> tobsI;                 //   phase | pressure | queue | 5 movement columns | phase pressure | lane scratch |
+                                       //   movement begin | movement intersection | phase count
+    DevBuf<double> tobsD;              //   phase remaining
+    DevBuf<unsigned char> tobsMv;      //   phase movements
+    IntObsTable tobs{};
+    DeviceIntersectionObs tobsOut{};
+    int *hPhaseFlush[RING] = {};       //   pinned staging of the setPhase calls a refresh sends up, one per ring slot ...
+    cudaEvent_t phaseFlushDone[RING] = {};   // ... free again once its copy has run
+    int phaseFlushIdx = 0;
+    cudaEvent_t tobsReady = nullptr, tobsConsumed = nullptr;
     std::vector<cudaEvent_t> stepEv;   // timed-step brackets (bench)
     size_t stepEvUsed = 0;
     DevBuf<unsigned char> flushBuf;
@@ -683,6 +700,8 @@ DeviceSim::~DeviceSim() {
         if (I.hSpawn[r]) cudaFreeHost(I.hSpawn[r]);
         if (I.spawnDone[r]) cudaEventDestroy(I.spawnDone[r]);
         if (I.hPhaseRing[r]) cudaFreeHost(I.hPhaseRing[r]);
+        if (I.hPhaseFlush[r]) cudaFreeHost(I.hPhaseFlush[r]);
+        if (I.phaseFlushDone[r]) cudaEventDestroy(I.phaseFlushDone[r]);
     }
     for (auto &ev : I.ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : I.stepEv) cudaEventDestroy(ev);
@@ -1361,6 +1380,51 @@ void DeviceSim::setCustomSpeedsFromDevice(const int32_t *slot, const int32_t *pr
     I.mirrorStale = true;    // k_vspeed may raise ERR_VEHICLE_* outside a step
 }
 
+DeviceIntersectionObs DeviceSim::observeIntersections(void *consumerStream) {
+    Impl &I = *impl_;
+    View &V = I.V;
+    if (V.owned) throw std::runtime_error("observeIntersections: not available on one rank of a sharded run");
+    if (!I.tobsI.p) {   // first call: the static tables and the columns as they stand before a refresh
+        const IntObsLayout X = intObsLayout(I.L, V);
+        I.tobsStatic.upload(X.ints.empty() ? std::vector<int>(1, 0) : X.ints);
+        I.tobsI.upload(X.initialInts(V));
+        I.tobsD.upload(std::vector<double>(std::max(V.nInter, 1), 0.0));
+        I.tobsMv.upload(X.phaseMovements);
+        legacySync();
+        X.point(I.tobs, I.tobsStatic.p);
+        X.pointOut(I.tobs, I.tobsOut, V, I.tobsI.p, I.tobsD.p, I.tobsMv.p);
+        I.tobsOut.device = I.opt.device;
+        CFB_CUDA(cudaEventCreateWithFlags(&I.tobsReady, cudaEventDisableTiming));
+        CFB_CUDA(cudaEventCreateWithFlags(&I.tobsConsumed, cudaEventDisableTiming));
+    }
+    cudaStream_t cs = (cudaStream_t) consumerStream;
+    CFB_CUDA(cudaEventRecord(I.tobsConsumed, cs));         // the consumer's earlier reads finish before the refresh ...
+    CFB_CUDA(cudaStreamWaitEvent(I.stream, I.tobsConsumed, 0));
+    if (I.phaseDirty && V.nInter) {   // setPhase calls made since the last step act at once (trafficlight.cpp:39-41)
+        const int r = I.phaseFlushIdx;
+        I.phaseFlushIdx = (r + 1) % Impl::RING;
+        if (!I.hPhaseFlush[r]) {
+            CFB_CUDA(cudaMallocHost(&I.hPhaseFlush[r], V.nInter * sizeof(int)));
+            CFB_CUDA(cudaEventCreateWithFlags(&I.phaseFlushDone[r], cudaEventDisableTiming));
+        }
+        CFB_CUDA(cudaEventSynchronize(I.phaseFlushDone[r]));   // its copy of RING refreshes ago has run (never waits in practice)
+        memcpy(I.hPhaseFlush[r], I.hPhase.data(), V.nInter * sizeof(int));
+        CFB_CUDA(cudaMemcpyAsync(V.curPhase, I.hPhaseFlush[r], V.nInter * sizeof(int), cudaMemcpyHostToDevice, I.stream));
+        CFB_CUDA(cudaEventRecord(I.phaseFlushDone[r], I.stream));
+        I.phaseDirty = false;
+    }
+    if (I.tobs.nTl > 0) {
+        const int grid = (I.tobs.nTl + TOBS_WARPS - 1) / TOBS_WARPS;
+        k_tobs<<<grid, TOBS_WARPS * 32, 0, I.stream>>>(V, I.tobs);
+        CFB_CUDA(cudaGetLastError());
+        launches_ += 1;
+    }
+    CFB_CUDA(cudaEventRecord(I.tobsReady, I.stream));      // ... and its later reads see it, the host waiting for neither
+    CFB_CUDA(cudaStreamWaitEvent(cs, I.tobsReady, 0));
+    return I.tobsOut;
+}
+
+DeviceIntersectionObs observeIntersectionsOf(DeviceSim &dev, void *consumerStream) { return dev.observeIntersections(consumerStream); }
 DeviceVehObs observeVehiclesOf(DeviceSim &dev, void *consumerStream) { return dev.observeVehicles(consumerStream); }
 void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot, const int32_t *priority, const double *speed, long long n,
                        void *producerStream) {

@@ -121,6 +121,23 @@ struct DeviceVehObs {
     int device = 0;
 };
 
+// The per-intersection and per-movement observations (device_tlobs.cuh).  A movement is a roadLink, in RoadNet's global
+// roadLink order.  The dynamic columns are refreshed by observeIntersections; the static ones are written once.
+struct DeviceIntersectionObs {
+    const int32_t *phase = nullptr;                // nInter: current phase index, -1 for a virtual intersection
+    const double *phaseRemaining = nullptr;        // nInter: View::remain (0 for a virtual intersection)
+    const int32_t *pressure = nullptr, *queue = nullptr;   // nInter
+    const int32_t *movementIn = nullptr, *movementInWaiting = nullptr, *movementOut = nullptr, *movementInside = nullptr,
+                  *movementPressure = nullptr;     // nRL each
+    const int32_t *phasePressure = nullptr;        // nInter x maxPhases, INT32_MIN past the intersection's phase count
+    const int32_t *movementBegin = nullptr;        // static: nInter + 1
+    const int32_t *movementIntersection = nullptr; // static: nRL
+    const int32_t *phaseCount = nullptr;           // static: nInter
+    const uint8_t *phaseMovements = nullptr;       // static: nInter x maxPhases x maxMovements
+    int nInter = 0, nRL = 0, maxPhases = 0, maxMovements = 0;
+    int device = 0;
+};
+
 class DeviceSim {
 public:
     // Throws std::runtime_error when no CUDA device / extension is usable (no CPU fallback).
@@ -185,6 +202,10 @@ public:
     // ERR_VEHICLE_STALE, a slot named twice ERR_VEHICLE_DUPLICATE.  No host synchronisation.
     void setCustomSpeedsFromDevice(const int32_t *slot, const int32_t *priority, const double *speed, long long n,
                                    void *producerStream);
+    // Every light's phase and every movement's queue and pressure, refreshed on the engine's stream with the same
+    // handshake as observeOnDevice, after the setPhase calls not yet sent to the device.  The buffers are made on the
+    // first call and keep their addresses for the engine's lifetime; their content is valid until the next call.
+    DeviceIntersectionObs observeIntersections(void *consumerStream);
     // Observations (synchronise the stream).
     int vehicleCount();
     int errorFlags();
@@ -272,5 +293,7 @@ private:
 __attribute__((weak)) DeviceVehObs observeVehiclesOf(DeviceSim &dev, void *consumerStream);
 __attribute__((weak)) void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot, const int32_t *priority, const double *speed,
                                              long long n, void *producerStream);
+// DeviceSim::observeIntersections, weak for the same reason.
+__attribute__((weak)) DeviceIntersectionObs observeIntersectionsOf(DeviceSim &dev, void *consumerStream);
 
 }  // namespace cfb

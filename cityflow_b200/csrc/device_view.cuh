@@ -141,6 +141,8 @@ __device__ __forceinline__ int x86int(double x) {
     return (x > -2147483649.0 && x < 2147483648.0) ? (int) x : INT_MIN;
 }
 constexpr double kEps = 1e-8;
+// Engine::getLaneWaitingVehicleCount engine.cpp:636-648: a vehicle slower than 0.1 m/s is waiting
+__device__ __forceinline__ bool isWaiting(double speed) { return speed < 0.1; }
 
 // Vehicle::getNoCollisionSpeed vehicle.cpp:200-209
 __device__ __forceinline__ double noCollisionSpeed(double vL, double dL, double vF, double dF, double gap, double dt,

@@ -1405,6 +1405,40 @@ const char *cfb_drivable_id(cfb_engine *e, int64_t d) {
     return e->drivableIds[d].c_str();
 }
 
+int cfb_observe_intersections_device(cfb_engine *e, void *consumer_stream, cfb_device_intersection_obs *out) {
+    if (!out) { e->lastError = "null output"; return CFB_ERR_ARGUMENT; }
+    CFB_TRY(e,
+        // (weak: a DeviceSim build without it -- the emulated device of the CPU suite -- leaves it null)
+        if (!cfb::observeIntersectionsOf)
+            throw std::runtime_error("intersection device observations are not part of this DeviceSim build");
+        const cfb::DeviceIntersectionObs o = cfb::observeIntersectionsOf(*e->h.dev, consumer_stream);
+        out->phase = o.phase; out->phase_remaining = o.phaseRemaining; out->pressure = o.pressure; out->queue = o.queue;
+        out->movement_in = o.movementIn; out->movement_in_waiting = o.movementInWaiting; out->movement_out = o.movementOut;
+        out->movement_inside = o.movementInside; out->movement_pressure = o.movementPressure;
+        out->phase_pressure = o.phasePressure;
+        out->movement_begin = o.movementBegin; out->movement_intersection = o.movementIntersection;
+        out->phase_count = o.phaseCount; out->phase_movements = o.phaseMovements;
+        out->n_intersections = o.nInter; out->n_road_links = o.nRL;
+        out->max_phases = o.maxPhases; out->max_movements = o.maxMovements;
+        out->device = o.device;
+    )
+    return CFB_OK;
+}
+
+int cfb_num_road_links(const cfb_engine *e) { return e->h.net.nRoadLinks(); }
+
+int cfb_road_link_info(const cfb_engine *e, int r, cfb_road_link *out) {
+    const cfb::RoadNet &n = e->h.net;
+    if (r < 0 || r >= n.nRoadLinks() || !out) return CFB_ERR_ARGUMENT;
+    out->intersection = n.rlInter[r];
+    out->index = r - n.interRoadLinkBeg[n.rlInter[r]];
+    out->type = n.rlType[r];
+    out->pad = 0;
+    out->start_road = n.roadId[n.rlStartRoad[r]].c_str();
+    out->end_road = n.roadId[n.rlEndRoad[r]].c_str();
+    return CFB_OK;
+}
+
 int64_t cfb_get_vehicle_speed(cfb_engine *e, cfb_vehicle_ref *ids, double *speed, double *distance, int64_t cap) {
     CFB_TRY(e,
         cfb::HostEngine &h = e->h;

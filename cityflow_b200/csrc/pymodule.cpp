@@ -177,6 +177,49 @@ public:
         d["device"] = py::int_(o.device);
         return d;
     }
+    // device pointers of the per-intersection / per-movement observations, ordered against CUDA stream `stream`
+    py::dict observeIntersectionsDevice(uintptr_t stream) {
+        cfb_device_intersection_obs o{};
+        check(cfb_observe_intersections_device(e_, (void *) stream, &o));
+        py::dict d;
+        d["phase"] = py::int_((uintptr_t) o.phase);
+        d["phase_remaining"] = py::int_((uintptr_t) o.phase_remaining);
+        d["pressure"] = py::int_((uintptr_t) o.pressure);
+        d["queue"] = py::int_((uintptr_t) o.queue);
+        d["movement_in"] = py::int_((uintptr_t) o.movement_in);
+        d["movement_in_waiting"] = py::int_((uintptr_t) o.movement_in_waiting);
+        d["movement_out"] = py::int_((uintptr_t) o.movement_out);
+        d["movement_inside"] = py::int_((uintptr_t) o.movement_inside);
+        d["movement_pressure"] = py::int_((uintptr_t) o.movement_pressure);
+        d["phase_pressure"] = py::int_((uintptr_t) o.phase_pressure);
+        d["movement_begin"] = py::int_((uintptr_t) o.movement_begin);
+        d["movement_intersection"] = py::int_((uintptr_t) o.movement_intersection);
+        d["phase_count"] = py::int_((uintptr_t) o.phase_count);
+        d["phase_movements"] = py::int_((uintptr_t) o.phase_movements);
+        d["n_intersections"] = py::int_(o.n_intersections);
+        d["n_road_links"] = py::int_(o.n_road_links);
+        d["max_phases"] = py::int_(o.max_phases);
+        d["max_movements"] = py::int_(o.max_movements);
+        d["device"] = py::int_(o.device);
+        return d;
+    }
+    // one dict per movement (roadLink), in the order of the movement columns
+    py::list roadLinks() {
+        static const char *types[] = {"", "turn_right", "turn_left", "go_straight"};
+        py::list out;
+        for (int r = 0; r < cfb_num_road_links(e_); ++r) {
+            cfb_road_link l{};
+            check(cfb_road_link_info(e_, r, &l));
+            py::dict d;
+            d["intersection"] = py::str(cfb_intersection_id(e_, l.intersection));
+            d["index"] = py::int_(l.index);
+            d["start_road"] = py::str(l.start_road);
+            d["end_road"] = py::str(l.end_road);
+            d["type"] = py::str(l.type >= 1 && l.type <= 3 ? types[l.type] : "");
+            out.append(d);
+        }
+        return out;
+    }
     // the reference's ids of vehicle slots (None: the slot holds no vehicle)
     py::list vehicleIds(const std::vector<int32_t> &slots) {
         std::vector<cfb_vehicle_ref> refs(slots.size());
@@ -411,6 +454,8 @@ PYBIND11_MODULE(_cityflow_b200, m) {
         .def("device", [](Engine &e) { return cfb_device(e.raw()); })
         .def("observe_device", &Engine::observeDevice, "stream"_a = 0)
         .def("observe_vehicles_device", &Engine::observeVehiclesDevice, "stream"_a = 0)
+        .def("observe_intersections_device", &Engine::observeIntersectionsDevice, "stream"_a = 0)
+        .def("road_links", &Engine::roadLinks)
         .def("set_vehicle_speeds_device", [](Engine &e, uintptr_t slot, uintptr_t priority, uintptr_t speed, int64_t n, uintptr_t stream) {
             if (cfb_set_vehicle_speeds_device(e.raw(), (const int32_t *) slot, (const int32_t *) priority, (const double *) speed, n,
                                               (void *) stream) < 0)

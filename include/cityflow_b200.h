@@ -140,6 +140,50 @@ int cfb_vehicle_refs(cfb_engine *e, const int32_t *slots, int64_t n, cfb_vehicle
 /* id of drivable d: lane ids first (cfb_lane_id), then laneLinks as "<start lane>_TO_<end lane>" (roadnet.h:478);
  * NULL when out of range */
 const char *cfb_drivable_id(cfb_engine *e, int64_t d);
+/* Per-intersection and per-movement observations left ON THE DEVICE, for a signal controller on the same GPU
+ * (MaxPressure, PressLight): refreshed and ordered against `consumer_stream` exactly as cfb_observe_device, after
+ * every cfb_set_tl_phase(_index) call made before it.  A movement is a roadLink: index r runs over the intersections
+ * in cfb_intersection_id order and, within one, over its "roadLinks" array (cfb_road_link_info); virtual
+ * intersections have none.  in_lanes(r) / out_lanes(r) are the distinct start / end lanes of r's laneLinks,
+ * in_lanes(i) / out_lanes(i) their union over intersection i's roadLinks; count(l) is what
+ * cfb_get_lane_vehicle_count reports (lane-change shadows included), waiting(l) what
+ * cfb_get_lane_waiting_vehicle_count reports.  The pointers stay valid for the engine's lifetime; the content of
+ * the dynamic columns is valid until the next call.  Single-GPU engines only. */
+typedef struct {
+    const int32_t *phase;                 /* [n_intersections] current phase index (cfb_set_tl_phase's); -1 virtual */
+    const double *phase_remaining;        /* [n_intersections] remainDuration as the JSON archive writes it; 0 virtual */
+    const int32_t *pressure;              /* [n_intersections] sum of count over in_lanes(i) - over out_lanes(i) */
+    const int32_t *queue;                 /* [n_intersections] sum of waiting over in_lanes(i) */
+    const int32_t *movement_in;           /* [n_road_links] sum of count over in_lanes(r) */
+    const int32_t *movement_in_waiting;   /* [n_road_links] sum of waiting over in_lanes(r) */
+    const int32_t *movement_out;          /* [n_road_links] sum of count over out_lanes(r) */
+    const int32_t *movement_inside;       /* [n_road_links] vehicles on r's laneLinks (shadows included) */
+    const int32_t *movement_pressure;     /* [n_road_links] movement_in - movement_out */
+    const int32_t *phase_pressure;        /* [n_intersections x max_phases] entry [i, k < phase_count[i]]: sum of
+                                             movement_pressure over the roadLinks available in phase k; INT32_MIN after */
+    const int32_t *movement_begin;        /* static [n_intersections + 1]: the movements of i are [begin[i], begin[i+1]) */
+    const int32_t *movement_intersection; /* static [n_road_links] */
+    const int32_t *phase_count;           /* static [n_intersections] light phases; 0 virtual */
+    const uint8_t *phase_movements;       /* static [n_intersections x max_phases x max_movements]: 1 where movement
+                                             begin[i] + m is available in phase k */
+    int32_t n_intersections;
+    int32_t n_road_links;
+    int32_t max_phases;                   /* at least 1 */
+    int32_t max_movements;                /* at least 1 */
+    int32_t device;                       /* CUDA device ordinal the pointers live on */
+} cfb_device_intersection_obs;
+int cfb_observe_intersections_device(cfb_engine *e, void *consumer_stream, cfb_device_intersection_obs *out);
+/* number of roadLinks (movements) of the roadnet: the length of cfb_device_intersection_obs's movement columns */
+int cfb_num_road_links(const cfb_engine *e);
+/* movement r as the roadnet file lists it; the road ids stay valid for the engine's lifetime */
+typedef struct {
+    int32_t intersection;                 /* cfb_intersection_id index */
+    int32_t index;                        /* position in the intersection's "roadLinks" array */
+    int32_t type;                         /* 1 turn_right, 2 turn_left, 3 go_straight (roadnet.h:401-403) */
+    int32_t pad;
+    const char *start_road, *end_road;
+} cfb_road_link;
+int cfb_road_link_info(const cfb_engine *e, int r, cfb_road_link *out);
 /* Engine::getVehicleSpeed  engine.cpp:662-668 / getVehicleDistance :670-676: running vehicles in
  * vehiclePool (priority) order.  Returns the number of running vehicles (may exceed cap; only
  * cap entries are written); any of the three output pointers may be NULL. */

@@ -6,7 +6,7 @@
 
 Small networks so the instrumented kernels finish in seconds: single engine (step kernels, spawn
 ring, observation kernels, archive, vehicle setters, the per-vehicle table and batched custom speed), rlTrafficLight engine (host and device phase
-setting, device-resident observations), lane change (its per-road
+setting, device-resident observations, the intersection observations with pending host phases), lane change (its per-road
 kernels run roads concurrently: racecheck is the interesting tool there) and a 2-rank loop-back shard group
 (pack/unpack/seal kernels).
 Exit code 0 and the sanitizer's "ERROR SUMMARY: 0 errors" are the result."""
@@ -67,6 +67,7 @@ def main():
             raise RuntimeError("SAN_NO_TORCH=1")
         import torch
         obs = cityflow_b200.LaneObservations(rl)
+        tobs = cityflow_b200.IntersectionObservations(rl)
         idx = torch.arange(rl.num_intersections(), device="cuda", dtype=torch.int32)
     except Exception as e:  # noqa: BLE001
         obs = None
@@ -81,6 +82,9 @@ def main():
                     rl.set_tl_phase(i, (t // 7) % 8)
                 except RuntimeError:
                     pass  # virtual intersection
+            if obs is not None:   # the refresh sends the pending set_tl_phase calls up first (device_tlobs.cuh)
+                tobs.refresh()
+                cityflow_b200.set_tl_phases_tensor(rl, tobs.phase_pressure.argmax(1).to(torch.int32))
         rl.next_step()
     print("rl ok, vehicles", rl.get_vehicle_count())
 
