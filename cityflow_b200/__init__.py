@@ -99,15 +99,37 @@ class VehicleObservations:
     engine's stream, ordered against ``stream`` (default: torch's current stream on that device) in both
     directions, without a host copy or wait; the tensors alias the engine's buffers and keep their storage
     across refreshes.  ``clone()`` what must survive the next refresh.  Single-GPU engines only.
+
+    With ``context=True`` every refresh also fills, from the same state, what lies ahead of each row (capacity
+    length, aligned with the rows):
+
+    * ``leader`` (int32): the row of the vehicle's leader as the last step found it (``get_leader``), which may
+      be on the next lane or on an overlapping laneLink; -1 none.
+    * ``gap`` (float64): the gap to that leader, bit-equal to the reference's; ``+inf`` without a leader.
+    * ``next_drivable`` (int32): the drivable the vehicle takes next, in ``drivable_ids`` numbering -- for a lane
+      row the laneLink it will take, for a laneLink row its end lane; -1 on the route's last road, -2 on a lane
+      that cannot continue the route.
+    * ``signal`` (int8): for a lane row heading for a laneLink, 1 if that movement is green in its
+      intersection's current phase (including ``set_tl_phase`` calls made since the last step), else 0; -1 on
+      every other row.
+
+    Padding rows hold leader -1, gap ``+inf``, next_drivable -1 and signal -1.  A lane-change shadow's row holds
+    the shadow's own leader, gap and next drivable, while ``get_leader`` of a shadow answers for its car.  Static
+    columns, aliases of the engine's tables: ``drivable_length`` and ``drivable_max_speed`` (float64, per
+    drivable; a laneLink's max speed is the reference's placeholder 10000) and ``link_road_link`` (int32, per
+    laneLink: the movement index of :class:`IntersectionObservations`).  ``n_lanes`` is where the laneLinks'
+    drivable numbers start.
     """
 
     _COLUMNS = (("slot", "<i4"), ("priority", "<i4"), ("drivable", "<i4"), ("distance", "<f8"), ("speed", "<f8"),
                 ("shadow", "|u1"))
+    _CONTEXT = (("leader", "<i4"), ("gap", "<f8"), ("next_drivable", "<i4"), ("signal", "|i1"))
 
-    def __init__(self, engine, stream=None):
+    def __init__(self, engine, stream=None, context=False):
         self.engine = engine
         self._device = engine.device()
         self._ptrs = None
+        self._context = context
         self.drivable_ids = engine.drivable_ids()
         self.refresh(stream)
 
@@ -118,16 +140,26 @@ class VehicleObservations:
         return int(getattr(stream, "cuda_stream", stream))
 
     def refresh(self, stream=None):
-        o = self.engine.observe_vehicles_device(self._stream(stream))
-        ptrs = tuple(o[k] for k, _ in self._COLUMNS) + (o["drivable_begin"], o["count"], o["capacity"])
+        if self._context:
+            o = self.engine.observe_vehicle_context_device(self._stream(stream))
+            columns = self._COLUMNS + self._CONTEXT
+        else:
+            o = self.engine.observe_vehicles_device(self._stream(stream))
+            columns = self._COLUMNS
+        ptrs = tuple(o[k] for k, _ in columns) + (o["drivable_begin"], o["count"], o["capacity"])
         if ptrs != self._ptrs:   # first call, or the engine re-allocated its buffers
             import torch
             dev = torch.device("cuda", o["device"])
             mk = lambda ptr, n, ts: torch.as_tensor(_DeviceArray(self.engine, ptr, n, ts), device=dev)  # noqa: E731
-            for k, ts in self._COLUMNS:
+            for k, ts in columns:
                 setattr(self, k, mk(o[k], o["capacity"], ts))
             self.drivable_begin = mk(o["drivable_begin"], o["n_drivables"] + 1, "<i4")
             self.count = mk(o["count"], 1, "<i4")
+            if self._context:
+                self.drivable_length = mk(o["drivable_length"], o["n_drivables"], "<f8")
+                self.drivable_max_speed = mk(o["drivable_max_speed"], o["n_drivables"], "<f8")
+                self.link_road_link = mk(o["link_road_link"], o["n_links"], "<i4")
+                self.n_lanes = o["n_lanes"]
             self._ptrs = ptrs
         return self
 

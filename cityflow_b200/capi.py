@@ -127,6 +127,7 @@ def bind(lib: ctypes.CDLL) -> ctypes.CDLL:
         "cfb_observe_intersections_device": (i32, [vp, vp, vp]),
         "cfb_num_road_links": (i32, [vp]),
         "cfb_road_link_info": (i32, [vp, i32, vp]),
+        "cfb_observe_vehicle_context_device": (i32, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         if not hasattr(lib, name):
@@ -143,6 +144,13 @@ class DeviceVehicleObs(ctypes.Structure):
                 ("distance", ctypes.c_void_p), ("speed", ctypes.c_void_p), ("shadow", ctypes.c_void_p),
                 ("drivable_begin", ctypes.c_void_p), ("count", ctypes.c_void_p), ("capacity", ctypes.c_int64),
                 ("n_drivables", ctypes.c_int32), ("device", ctypes.c_int32)]
+
+
+class DeviceVehicleContext(ctypes.Structure):
+    """cfb_device_vehicle_context: the per-vehicle table and what lies ahead of each row (include/cityflow_b200.h)."""
+    _fields_ = [("table", DeviceVehicleObs)] + [(k, ctypes.c_void_p) for k in (
+        "leader", "gap", "next_drivable", "signal", "drivable_length", "drivable_max_speed", "link_road_link")] + \
+        [("n_lanes", ctypes.c_int32), ("n_links", ctypes.c_int32)]
 
 
 class DeviceIntersectionObs(ctypes.Structure):
@@ -324,6 +332,13 @@ class CEngine:
     def set_vehicle_speeds_device(self, slot: int, priority: int, speed: int, n: int, stream: int = 0):
         """cfb_set_vehicle_speeds_device: slot / priority / speed are device addresses of n entries each."""
         self._check(self.lib.cfb_set_vehicle_speeds_device(self.h, slot, priority, speed, n, stream))
+
+    def observe_vehicle_context_device(self, stream: int = 0) -> DeviceVehicleContext:
+        """Refresh the per-vehicle table with each row's leader, gap, next drivable and light
+        (cfb_observe_vehicle_context_device) and return their pointers."""
+        o = DeviceVehicleContext()
+        self._check(self.lib.cfb_observe_vehicle_context_device(self.h, stream, ctypes.byref(o)))
+        return o
 
     def observe_intersections_device(self, stream: int = 0) -> DeviceIntersectionObs:
         """Refresh the intersection observations (cfb_observe_intersections_device) and return their pointers."""

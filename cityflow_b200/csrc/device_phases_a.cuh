@@ -93,9 +93,7 @@ __device__ __forceinline__ void phase_ingest(const View &V, const int bid, const
     const int nRLmine = V.ingRL ? V.nIngRL : V.nRL;
     for (int x = i; x < nRLmine; x += nblk * blockDim.x) {
         const int r = V.ingRL ? V.ingRL[x] : x;
-        int in = V.rlInter[r];
-        int ph = V.interPhaseBeg[in] + V.curPhase[in];
-        V.rlAvail[r] = V.phaseAvail[V.phaseAvailBeg[ph] + (r - V.interRLBeg[in])];
+        V.rlAvail[r] = roadLinkAvailable(V, r);
     }
     if (V.ingLinks) {
         for (int x = i; x < V.nIngLinks * V.maskWords; x += nblk * blockDim.x)

@@ -197,6 +197,8 @@ namespace cfb {
 // The per-vehicle table (device_vehobs.cuh): tile sums, then offsets + bucket copies.  And the batched custom speed.
 __global__ void __launch_bounds__(VOBS_TILE) k_vobs_sums(View V, VehObsTable T) { vobsTileSums(V, T, blockIdx.x); }
 __global__ void __launch_bounds__(VOBS_TILE) k_vobs_fill(View V, VehObsTable T) { vobsFill(V, T, blockIdx.x, gridDim.x); }
+// What lies ahead of every row (leader, gap, next drivable, light), one thread per row after the two above.
+__global__ void __launch_bounds__(256) k_vctx(View V, VehObsTable T, VehCtxTable C) { vctxFill(V, T, C, blockIdx.x, gridDim.x); }
 __global__ void __launch_bounds__(256) k_vspeed(View V, const int *slot, const int *priority, const double *speed, int n,
                                                 int *stamp, int slotCap, int call) {
     vspeedApply(V, slot, priority, speed, n, stamp, slotCap, call, blockIdx.x, gridDim.x);
@@ -393,6 +395,10 @@ struct DeviceSim::Impl {
     VehObsTable vobs{};
     int vobsTiles = 0;
     cudaEvent_t vobsReady = nullptr, vobsConsumed = nullptr;
+    DevBuf<int> vctxI;                 // observeVehicleContext(): leader | next drivable (capacity rows each), mark (2)
+    DevBuf<double> vctxGap;
+    DevBuf<signed char> vctxSignal;
+    VehCtxTable vctx{};
     DevBuf<int> speedStamp;            // setCustomSpeedsFromDevice(): per slot, the last call that named it
     int speedCall = 0;
     cudaEvent_t speedReady = nullptr, speedTaken = nullptr;
@@ -1304,13 +1310,31 @@ DeviceObs DeviceSim::observeOnDevice(void *consumerStream) {
     return o;
 }
 
-DeviceVehObs DeviceSim::observeVehicles(void *consumerStream) {
-    Impl &I = *impl_;
-    if (I.V.owned) throw std::runtime_error("observeVehicles: not available on one rank of a sharded run");
+// setPhase calls made since the last step act at once (trafficlight.cpp:39-41): a refresh that reads the phases sends
+// them up first, on the engine's stream, through a ring of pinned buffers each guarded by the event of its last copy.
+static void sendPendingPhases(DeviceSim::Impl &I) {
+    View &V = I.V;
+    if (!I.phaseDirty || !V.nInter) return;
+    const int r = I.phaseFlushIdx;
+    I.phaseFlushIdx = (r + 1) % DeviceSim::Impl::RING;
+    if (!I.hPhaseFlush[r]) {
+        CFB_CUDA(cudaMallocHost(&I.hPhaseFlush[r], V.nInter * sizeof(int)));
+        CFB_CUDA(cudaEventCreateWithFlags(&I.phaseFlushDone[r], cudaEventDisableTiming));
+    }
+    CFB_CUDA(cudaEventSynchronize(I.phaseFlushDone[r]));   // its copy of RING refreshes ago has run (never waits in practice)
+    memcpy(I.hPhaseFlush[r], I.hPhase.data(), V.nInter * sizeof(int));
+    CFB_CUDA(cudaMemcpyAsync(V.curPhase, I.hPhaseFlush[r], V.nInter * sizeof(int), cudaMemcpyHostToDevice, I.stream));
+    CFB_CUDA(cudaEventRecord(I.phaseFlushDone[r], I.stream));
+    I.phaseDirty = false;
+}
+
+// The per-vehicle table's buffers, made on the first refresh (the row capacity is the position capacity, fixed when the
+// engine is made), and the pointers a refresh hands out.
+static void vobsMake(DeviceSim::Impl &I) {
     const size_t cap = (size_t) std::max(I.P, 1), nD = (size_t) I.V.nDrv;
     const int tiles = (int) std::max<size_t>(1, (nD + VOBS_TILE - 1) / VOBS_TILE);
     const size_t nI = 3 * cap + (nD + 1) + 2 + (size_t) tiles;
-    if (I.vobsI.n < nI) {   // first call (the row capacity is the position capacity, fixed when the engine is made)
+    if (I.vobsI.n < nI) {
         I.vobsI.alloc(nI);
         I.vobsD.alloc(2 * cap);
         I.vobsShadow.alloc(cap);
@@ -1328,6 +1352,23 @@ DeviceVehObs DeviceSim::observeVehicles(void *consumerStream) {
             CFB_CUDA(cudaEventCreateWithFlags(&I.vobsConsumed, cudaEventDisableTiming));
         }
     }
+}
+static DeviceVehObs vobsOut(const DeviceSim::Impl &I) {
+    const VehObsTable &T = I.vobs;
+    DeviceVehObs o;
+    o.slot = T.slot; o.priority = T.priority; o.drivable = T.drivable;
+    o.distance = T.distance; o.speed = T.speed; o.shadow = T.shadow;
+    o.drivableBegin = T.drvBegin; o.count = T.count;
+    o.capacity = (long long) std::max(I.P, 1);
+    o.nDrv = I.V.nDrv;
+    o.device = I.opt.device;
+    return o;
+}
+
+DeviceVehObs DeviceSim::observeVehicles(void *consumerStream) {
+    Impl &I = *impl_;
+    if (I.V.owned) throw std::runtime_error("observeVehicles: not available on one rank of a sharded run");
+    vobsMake(I);
     cudaStream_t cs = (cudaStream_t) consumerStream;
     CFB_CUDA(cudaEventRecord(I.vobsConsumed, cs));         // the consumer's earlier reads finish before the refresh ...
     CFB_CUDA(cudaStreamWaitEvent(I.stream, I.vobsConsumed, 0));
@@ -1337,14 +1378,45 @@ DeviceVehObs DeviceSim::observeVehicles(void *consumerStream) {
     CFB_CUDA(cudaEventRecord(I.vobsReady, I.stream));      // ... and its later reads see it, the host waiting for neither
     CFB_CUDA(cudaStreamWaitEvent(cs, I.vobsReady, 0));
     launches_ += 2;
-    const VehObsTable &T = I.vobs;
-    DeviceVehObs o;
-    o.slot = T.slot; o.priority = T.priority; o.drivable = T.drivable;
-    o.distance = T.distance; o.speed = T.speed; o.shadow = T.shadow;
-    o.drivableBegin = T.drvBegin; o.count = T.count;
-    o.capacity = (long long) cap;
-    o.nDrv = I.V.nDrv;
-    o.device = I.opt.device;
+    return vobsOut(I);
+}
+
+DeviceVehCtx DeviceSim::observeVehicleContext(void *consumerStream) {
+    Impl &I = *impl_;
+    View &V = I.V;
+    if (V.owned) throw std::runtime_error("observeVehicleContext: not available on one rank of a sharded run");
+    vobsMake(I);
+    const size_t cap = (size_t) std::max(I.P, 1);
+    if (!I.vctxI.p) {   // first call: every row counts as filled, so the first refresh writes the padding of all of them
+        std::vector<int> ints(2 * cap + 2, -1);
+        ints[2 * cap] = ints[2 * cap + 1] = (int) cap;
+        I.vctxI.upload(ints);
+        I.vctxGap.alloc(cap);
+        I.vctxSignal.alloc(cap);
+        legacySync();
+        VehCtxTable &C = I.vctx;
+        C.leader = I.vctxI.p; C.nextDrivable = C.leader + cap; C.mark = C.nextDrivable + cap; C.par = 0;
+        C.gap = I.vctxGap.p; C.signal = I.vctxSignal.p;
+    }
+    cudaStream_t cs = (cudaStream_t) consumerStream;
+    CFB_CUDA(cudaEventRecord(I.vobsConsumed, cs));         // the consumer's earlier reads finish before the refresh ...
+    CFB_CUDA(cudaStreamWaitEvent(I.stream, I.vobsConsumed, 0));
+    sendPendingPhases(I);
+    k_vobs_sums<<<I.vobsTiles, VOBS_TILE, 0, I.stream>>>(V, I.vobs);
+    k_vobs_fill<<<I.vobsTiles, VOBS_TILE, 0, I.stream>>>(V, I.vobs);
+    const int grid = (int) std::min<size_t>((cap + 255) / 256, (size_t) I.numSMs * 8);
+    k_vctx<<<grid, 256, 0, I.stream>>>(V, I.vobs, I.vctx);
+    CFB_CUDA(cudaGetLastError());
+    I.vctx.par ^= 1;
+    CFB_CUDA(cudaEventRecord(I.vobsReady, I.stream));      // ... and its later reads see it, the host waiting for neither
+    CFB_CUDA(cudaStreamWaitEvent(cs, I.vobsReady, 0));
+    launches_ += 3;
+    DeviceVehCtx o;
+    o.table = vobsOut(I);
+    const VehCtxTable &C = I.vctx;
+    o.leader = C.leader; o.gap = C.gap; o.nextDrivable = C.nextDrivable; o.signal = C.signal;
+    o.drivableLength = V.drvLength; o.drivableMaxSpeed = V.drvMaxSpeed; o.linkRoadLink = V.llRoadLink;
+    o.nLanes = V.nLanes; o.nLinks = V.nLinks;
     return o;
 }
 
@@ -1400,19 +1472,7 @@ DeviceIntersectionObs DeviceSim::observeIntersections(void *consumerStream) {
     cudaStream_t cs = (cudaStream_t) consumerStream;
     CFB_CUDA(cudaEventRecord(I.tobsConsumed, cs));         // the consumer's earlier reads finish before the refresh ...
     CFB_CUDA(cudaStreamWaitEvent(I.stream, I.tobsConsumed, 0));
-    if (I.phaseDirty && V.nInter) {   // setPhase calls made since the last step act at once (trafficlight.cpp:39-41)
-        const int r = I.phaseFlushIdx;
-        I.phaseFlushIdx = (r + 1) % Impl::RING;
-        if (!I.hPhaseFlush[r]) {
-            CFB_CUDA(cudaMallocHost(&I.hPhaseFlush[r], V.nInter * sizeof(int)));
-            CFB_CUDA(cudaEventCreateWithFlags(&I.phaseFlushDone[r], cudaEventDisableTiming));
-        }
-        CFB_CUDA(cudaEventSynchronize(I.phaseFlushDone[r]));   // its copy of RING refreshes ago has run (never waits in practice)
-        memcpy(I.hPhaseFlush[r], I.hPhase.data(), V.nInter * sizeof(int));
-        CFB_CUDA(cudaMemcpyAsync(V.curPhase, I.hPhaseFlush[r], V.nInter * sizeof(int), cudaMemcpyHostToDevice, I.stream));
-        CFB_CUDA(cudaEventRecord(I.phaseFlushDone[r], I.stream));
-        I.phaseDirty = false;
-    }
+    sendPendingPhases(I);
     if (I.tobs.nTl > 0) {
         const int grid = (I.tobs.nTl + TOBS_WARPS - 1) / TOBS_WARPS;
         k_tobs<<<grid, TOBS_WARPS * 32, 0, I.stream>>>(V, I.tobs);
@@ -1426,6 +1486,7 @@ DeviceIntersectionObs DeviceSim::observeIntersections(void *consumerStream) {
 
 DeviceIntersectionObs observeIntersectionsOf(DeviceSim &dev, void *consumerStream) { return dev.observeIntersections(consumerStream); }
 DeviceVehObs observeVehiclesOf(DeviceSim &dev, void *consumerStream) { return dev.observeVehicles(consumerStream); }
+DeviceVehCtx observeVehicleContextOf(DeviceSim &dev, void *consumerStream) { return dev.observeVehicleContext(consumerStream); }
 void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot, const int32_t *priority, const double *speed, long long n,
                        void *producerStream) {
     dev.setCustomSpeedsFromDevice(slot, priority, speed, n, producerStream);

@@ -121,6 +121,19 @@ struct DeviceVehObs {
     int device = 0;
 };
 
+// What lies ahead of every row of the per-vehicle table (device_vehobs.cuh, VehCtxTable), refreshed together with the
+// table; capacity rows each, aligned with its rows.  The static arrays alias the engine's own tables.
+struct DeviceVehCtx {
+    DeviceVehObs table;
+    const int32_t *leader = nullptr;          // row of the leader, -1 none
+    const double *gap = nullptr;              // ControllerInfo::gap to it, +inf without a leader
+    const int32_t *nextDrivable = nullptr;    // Router::getNextDrivable; PLAN_END / PLAN_DEAD where there is none
+    const int8_t *signal = nullptr;           // a lane row heading for a laneLink: its roadLink available now (1) or not (0); else -1
+    const double *drivableLength = nullptr, *drivableMaxSpeed = nullptr;   // static: nDrv each
+    const int32_t *linkRoadLink = nullptr;    // static: nLinks
+    int nLanes = 0, nLinks = 0;
+};
+
 // The per-intersection and per-movement observations (device_tlobs.cuh).  A movement is a roadLink, in RoadNet's global
 // roadLink order.  The dynamic columns are refreshed by observeIntersections; the static ones are written once.
 struct DeviceIntersectionObs {
@@ -206,6 +219,10 @@ public:
     // handshake as observeOnDevice, after the setPhase calls not yet sent to the device.  The buffers are made on the
     // first call and keep their addresses for the engine's lifetime; their content is valid until the next call.
     DeviceIntersectionObs observeIntersections(void *consumerStream);
+    // The per-vehicle table (as observeVehicles) and, for every row, its leader, the gap to it, its next drivable and the
+    // light at its stop line, in one refresh with the same handshake, after the setPhase calls not yet sent to the
+    // device.  The buffers are made on the first call and keep their addresses; their content is valid until the next call.
+    DeviceVehCtx observeVehicleContext(void *consumerStream);
     // Observations (synchronise the stream).
     int vehicleCount();
     int errorFlags();
@@ -295,5 +312,7 @@ __attribute__((weak)) void setCustomSpeedsOf(DeviceSim &dev, const int32_t *slot
                                              long long n, void *producerStream);
 // DeviceSim::observeIntersections, weak for the same reason.
 __attribute__((weak)) DeviceIntersectionObs observeIntersectionsOf(DeviceSim &dev, void *consumerStream);
+// DeviceSim::observeVehicleContext, weak for the same reason.
+__attribute__((weak)) DeviceVehCtx observeVehicleContextOf(DeviceSim &dev, void *consumerStream);
 
 }  // namespace cfb

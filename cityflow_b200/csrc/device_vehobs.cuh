@@ -1,5 +1,6 @@
 // device_vehobs.cuh -- per-vehicle observations and actions for a consumer on the same GPU: the table of every running
-// vehicle (DeviceSim::observeVehicles) and the batched custom speed (DeviceSim::setCustomSpeedsFromDevice).  Kernel
+// vehicle (DeviceSim::observeVehicles), what lies ahead of each row (DeviceSim::observeVehicleContext) and the batched
+// custom speed (DeviceSim::setCustomSpeedsFromDevice).  Kernel
 // bodies only, written as (View, block, grid) functions, so that the emulated device (tests/device_sim_emu.cpp) runs the
 // same code as device_sim.cu.  Nothing here is part of a step.
 #pragma once
@@ -103,6 +104,62 @@ __device__ __forceinline__ void vobsFill(const View &V, const VehObsTable &T, in
     }
     const int prev = *T.prevCount;
     for (int r = total + b * blockDim.x + threadIdx.x; r < prev; r += nb * blockDim.x) T.slot[r] = -1;
+}
+
+// What lies ahead of every row of a VehObsTable, filled right after the table in the same refresh
+// (DeviceSim::observeVehicleContext).  Capacity rows each; rows at and beyond *T.count hold the padding values
+// leader -1, gap +inf, nextDrivable -1, signal -1.
+struct VehCtxTable {
+    int *leader;               // row of Vehicle::getLeader (View::leader), -1 none
+    double *gap;               // ControllerInfo::gap to it, +inf without a leader
+    int *nextDrivable;         // Router::getNextDrivable: ids[p].w (PLAN_END / PLAN_DEAD where there is none)
+    signed char *signal;       // a lane row heading for a laneLink: RoadLink::isAvailable of its roadLink (0 / 1); else -1
+    int *mark;                 // two entries: rows filled by the previous context refresh, read from mark[par] ...
+    int par;                   // ... and this refresh's row count written to mark[par ^ 1]
+};
+
+// One thread per row, grid-stride.  Row r of drivable d is position off[d] + (r - drvBegin[d]).  A leader one position
+// ahead on the same drivable is the row before; any other leader (the next lane, or an overlapping laneLink from the
+// same start lane, vehicle.cpp:157-190) is found by a binary search of View::off for its drivable.  The rows the
+// previous context refresh filled beyond the new count become padding again: that mark is kept here, apart from the
+// table's prevCount, which a refresh without the context also moves.
+__device__ __forceinline__ void vctxFill(const View &V, const VehObsTable &T, const VehCtxTable &C, int b, int nb) {
+    const int n = *T.count, mark = C.mark[C.par];
+    if (b == 0 && threadIdx.x == 0) C.mark[C.par ^ 1] = n;
+    const int end = n > mark ? n : mark;
+    for (int r = b * blockDim.x + threadIdx.x; r < end; r += nb * blockDim.x) {
+        if (r >= n) {
+            C.leader[r] = -1;
+            C.gap[r] = (double) INFINITY;
+            C.nextDrivable[r] = -1;
+            C.signal[r] = -1;
+            continue;
+        }
+        const int d = T.drivable[r], k = r - T.drvBegin[d], p = V.off[d] + k;
+        const int lp = V.leader[p];
+        int lr = -1;
+        double g = (double) INFINITY;
+        if (lp >= 0) {
+            if (k > 0 && lp == p - 1) {
+                lr = r - 1;
+            } else {
+                int lo = 0, hi = V.nDrv - 1;   // the last drivable whose bucket starts at or before lp
+                while (lo < hi) {
+                    const int mid = (lo + hi + 1) >> 1;
+                    if (V.off[mid] <= lp) lo = mid; else hi = mid - 1;
+                }
+                lr = T.drvBegin[lo] + (lp - V.off[lo]);
+            }
+            g = V.lcOn ? V.lc.slot[V.ids[p].x].gap : V.gap[p];
+        }
+        const int nd = V.ids[p].w;
+        signed char sig = -1;
+        if (d < V.nLanes && nd >= V.nLanes) sig = (signed char) roadLinkAvailable(V, V.llRoadLink[nd - V.nLanes]);
+        C.leader[r] = lr;
+        C.gap[r] = g;
+        C.nextDrivable[r] = nd;
+        C.signal[r] = sig;
+    }
 }
 
 // Vehicle::setCustomSpeed (vehicle.h:128) for every entry i with slot[i] >= 0, one thread per entry.  (slot, priority)

@@ -143,6 +143,12 @@ __device__ __forceinline__ int x86int(double x) {
 constexpr double kEps = 1e-8;
 // Engine::getLaneWaitingVehicleCount engine.cpp:636-648: a vehicle slower than 0.1 m/s is waiting
 __device__ __forceinline__ bool isWaiting(double speed) { return speed < 0.1; }
+// RoadLink::isAvailable roadnet.h:429-431: roadLink r is available in its intersection's current phase (View::curPhase)
+__device__ __forceinline__ unsigned char roadLinkAvailable(const View &V, int r) {
+    const int in = V.rlInter[r];
+    const int ph = V.interPhaseBeg[in] + V.curPhase[in];
+    return V.phaseAvail[V.phaseAvailBeg[ph] + (r - V.interRLBeg[in])];
+}
 
 // Vehicle::getNoCollisionSpeed vehicle.cpp:200-209
 __device__ __forceinline__ double noCollisionSpeed(double vL, double dL, double vF, double dF, double gap, double dt,

@@ -1359,17 +1359,36 @@ static void needVehicleObs() {
         throw std::runtime_error("per-vehicle device observations / actions are not part of this DeviceSim build");
 }
 
+static void vehicleObsOut(const cfb::DeviceVehObs &o, cfb_device_vehicle_obs *out) {
+    out->slot = o.slot; out->priority = o.priority; out->drivable = o.drivable;
+    out->distance = o.distance; out->speed = o.speed; out->shadow = o.shadow;
+    out->drivable_begin = o.drivableBegin; out->count = o.count;
+    out->capacity = o.capacity;
+    out->n_drivables = o.nDrv;
+    out->device = o.device;
+}
+
 int cfb_observe_vehicles_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_obs *out) {
     if (!out) { e->lastError = "null output"; return CFB_ERR_ARGUMENT; }
     CFB_TRY(e,
         needVehicleObs();
-        const cfb::DeviceVehObs o = cfb::observeVehiclesOf(*e->h.dev, consumer_stream);
-        out->slot = o.slot; out->priority = o.priority; out->drivable = o.drivable;
-        out->distance = o.distance; out->speed = o.speed; out->shadow = o.shadow;
-        out->drivable_begin = o.drivableBegin; out->count = o.count;
-        out->capacity = o.capacity;
-        out->n_drivables = o.nDrv;
-        out->device = o.device;
+        vehicleObsOut(cfb::observeVehiclesOf(*e->h.dev, consumer_stream), out);
+    )
+    return CFB_OK;
+}
+
+int cfb_observe_vehicle_context_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_context *out) {
+    if (!out) { e->lastError = "null output"; return CFB_ERR_ARGUMENT; }
+    CFB_TRY(e,
+        // (weak: a DeviceSim build without it -- the emulated device of the CPU suite -- leaves it null)
+        if (!cfb::observeVehicleContextOf)
+            throw std::runtime_error("per-vehicle device context is not part of this DeviceSim build");
+        const cfb::DeviceVehCtx o = cfb::observeVehicleContextOf(*e->h.dev, consumer_stream);
+        vehicleObsOut(o.table, &out->table);
+        out->leader = o.leader; out->gap = o.gap; out->next_drivable = o.nextDrivable; out->signal = o.signal;
+        out->drivable_length = o.drivableLength; out->drivable_max_speed = o.drivableMaxSpeed;
+        out->link_road_link = o.linkRoadLink;
+        out->n_lanes = o.nLanes; out->n_links = o.nLinks;
     )
     return CFB_OK;
 }

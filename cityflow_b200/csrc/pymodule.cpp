@@ -163,6 +163,25 @@ public:
     py::dict observeVehiclesDevice(uintptr_t stream) {
         cfb_device_vehicle_obs o{};
         check(cfb_observe_vehicles_device(e_, (void *) stream, &o));
+        return vehicleObsDict(o);
+    }
+    // the same table refreshed with what lies ahead of each row, and the static drivable / laneLink arrays
+    py::dict observeVehicleContextDevice(uintptr_t stream) {
+        cfb_device_vehicle_context o{};
+        check(cfb_observe_vehicle_context_device(e_, (void *) stream, &o));
+        py::dict d = vehicleObsDict(o.table);
+        d["leader"] = py::int_((uintptr_t) o.leader);
+        d["gap"] = py::int_((uintptr_t) o.gap);
+        d["next_drivable"] = py::int_((uintptr_t) o.next_drivable);
+        d["signal"] = py::int_((uintptr_t) o.signal);
+        d["drivable_length"] = py::int_((uintptr_t) o.drivable_length);
+        d["drivable_max_speed"] = py::int_((uintptr_t) o.drivable_max_speed);
+        d["link_road_link"] = py::int_((uintptr_t) o.link_road_link);
+        d["n_lanes"] = py::int_(o.n_lanes);
+        d["n_links"] = py::int_(o.n_links);
+        return d;
+    }
+    static py::dict vehicleObsDict(const cfb_device_vehicle_obs &o) {
         py::dict d;
         d["slot"] = py::int_((uintptr_t) o.slot);
         d["priority"] = py::int_((uintptr_t) o.priority);
@@ -454,6 +473,7 @@ PYBIND11_MODULE(_cityflow_b200, m) {
         .def("device", [](Engine &e) { return cfb_device(e.raw()); })
         .def("observe_device", &Engine::observeDevice, "stream"_a = 0)
         .def("observe_vehicles_device", &Engine::observeVehiclesDevice, "stream"_a = 0)
+        .def("observe_vehicle_context_device", &Engine::observeVehicleContextDevice, "stream"_a = 0)
         .def("observe_intersections_device", &Engine::observeIntersectionsDevice, "stream"_a = 0)
         .def("road_links", &Engine::roadLinks)
         .def("set_vehicle_speeds_device", [](Engine &e, uintptr_t slot, uintptr_t priority, uintptr_t speed, int64_t n, uintptr_t stream) {

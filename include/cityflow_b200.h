@@ -124,6 +124,38 @@ typedef struct {
     int32_t device;                  /* CUDA device ordinal the pointers live on */
 } cfb_device_vehicle_obs;
 int cfb_observe_vehicles_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_obs *out);
+/* What lies ahead of every vehicle, refreshed ON THE DEVICE together with the per-vehicle table: `table` is what
+ * cfb_observe_vehicles_device returns, refreshed by this call, and the four columns below have its capacity and its
+ * rows.  Ordered against `consumer_stream` as cfb_observe_device, after every cfb_set_tl_phase(_index) call made
+ * before it.  Row r holds:
+ *   leader         the row of Vehicle::getLeader as the last step left it; it may sit on another drivable (the next
+ *                  lane, or an overlapping laneLink from the same start lane, vehicle.cpp:157-190); -1 none
+ *   gap            ControllerInfo::gap to that leader (bit-equal to cfb_debug_vehicles'); +inf without a leader
+ *   next_drivable  Router::getNextDrivable in the table's drivable numbering: a lane row the laneLink it will take
+ *                  (n_lanes + k), a laneLink row its end lane; -1 on the route's last road, -2 where the lane cannot
+ *                  continue the route
+ *   signal         a lane row whose next drivable is a laneLink: 1 if that laneLink's roadLink is available in its
+ *                  intersection's current phase (RoadLink::isAvailable, the phase cfb_observe_intersections_device
+ *                  reports), else 0; -1 on every other row
+ * Padding rows (count to capacity): leader -1, gap +inf, next_drivable -1, signal -1.  A lane-change shadow's row
+ * holds the shadow's own leader, gap and next drivable (cfb_get_leader of a shadow answers for its car).  The static
+ * arrays alias the engine's tables: drivable_length and drivable_max_speed per drivable (a laneLink's max speed is the
+ * reference's placeholder 10000, roadnet.h:456), link_road_link per laneLink (the movement index of
+ * cfb_observe_intersections_device).  Pointers and content live as cfb_observe_vehicles_device's.  Single-GPU engines
+ * only. */
+typedef struct {
+    cfb_device_vehicle_obs table;
+    const int32_t *leader;
+    const double *gap;
+    const int32_t *next_drivable;
+    const int8_t *signal;
+    const double *drivable_length;       /* static [n_drivables] Drivable::getLength */
+    const double *drivable_max_speed;    /* static [n_drivables] Drivable::getMaxSpeed */
+    const int32_t *link_road_link;       /* static [n_links] */
+    int32_t n_lanes;
+    int32_t n_links;
+} cfb_device_vehicle_context;
+int cfb_observe_vehicle_context_device(cfb_engine *e, void *consumer_stream, cfb_device_vehicle_context *out);
 /* Engine::setVehicleSpeed (engine.cpp:827-834) for n vehicles at once, with the actions already ON THE DEVICE: slot,
  * priority (int32) and speed (double), n entries each in device memory, consumed on the engine's stream after the work
  * enqueued on `producer_stream` so far (as cfb_set_tl_phases_device).  Entries with slot < 0 are skipped, so the padded

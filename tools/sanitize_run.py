@@ -5,7 +5,7 @@
     compute-sanitizer --tool initcheck python tools/sanitize_run.py
 
 Small networks so the instrumented kernels finish in seconds: single engine (step kernels, spawn
-ring, observation kernels, archive, vehicle setters, the per-vehicle table and batched custom speed), rlTrafficLight engine (host and device phase
+ring, observation kernels, archive, vehicle setters, the per-vehicle table with and without its context and batched custom speed), rlTrafficLight engine (host and device phase
 setting, device-resident observations, the intersection observations with pending host phases), lane change (its per-road
 kernels run roads concurrently: racecheck is the interesting tool there) and a 2-rank loop-back shard group
 (pack/unpack/seal kernels).
@@ -56,6 +56,12 @@ def main():
         for _ in range(20):
             vo.refresh()
             cityflow_b200.set_vehicle_speeds_tensor(eng, vo.slot, vo.priority, (vo.speed * 0.5).contiguous())
+            eng.next_step()
+        vc = cityflow_b200.VehicleObservations(eng, context=True)   # what lies ahead of each row (k_vctx), plain refreshes between
+        for k in range(20):
+            vc.refresh()
+            if k % 2:
+                vo.refresh()
             eng.next_step()
         torch.cuda.synchronize()
         print("vehicle table ok, rows", int(vo.count.item()), eng.get_vehicle_count())
