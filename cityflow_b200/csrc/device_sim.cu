@@ -65,6 +65,7 @@ namespace cg = cooperative_groups;
 #include "device_layout.cuh"
 #include "device_phases_a.cuh"
 namespace cfb {
+static_assert(DeviceSim::LC_MAX_CANDIDATES == LC_MAX_CAND, "the host lends one spare slot per schedulable candidate");
 // Programmatic dependent launch: the five step kernels are chained with programmatic stream serialisation, so the next
 // kernel's launch, block scheduling and prologue overlap the tail of the previous one (each kernel is latency-bound and
 // drains unevenly).  `griddepcontrol.wait` returns once the whole previous grid has completed and its memory operations
@@ -1854,7 +1855,7 @@ void DeviceSim::stepLcBegin(const SpawnRec *recs, int n, const int32_t *spare, i
     CFB_CUDA(cudaMemcpyAsync(I.hLcCtrl, I.lcCtrl.p, sizeof(LcCtrl), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
     CFB_CUDA(cudaGetLastError());
-    if (I.hLcCtrl->error) throw std::runtime_error("cityflow_b200: lane-change capacity exceeded (candidates per step or spare slots)");
+    lcCheckCapacity(I.hLcCtrl->error);
     const int ns = I.hLcCtrl->nShadows;
     created.resize(ns);
     if (ns > 0) {

@@ -5,6 +5,7 @@
 // include it.
 #pragma once
 #include <cstdint>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -288,9 +289,20 @@ public:
     // allocate the lane-change state and upload its static tables (segments, lane geometry, lane plans)
     void enableLaneChange(const RoadNet &net, const Routing &routing);
     void uploadLanePlans(const Routing &routing);
+    // Candidates a step can schedule (LC_MAX_CAND, device_lc_types.cuh).  Each creates at most one shadow, so this
+    // many spare slots always suffice.
+    static constexpr int LC_MAX_CANDIDATES = 4096;
+    // Throws for the bits the lane-change kernels set in LcCtrl::error (device_lc.cuh, device_control.cuh).
+    static void lcCheckCapacity(int error) {
+        if (error & 1)
+            throw std::runtime_error("cityflow_b200: more than " + std::to_string(LC_MAX_CANDIDATES) +
+                                     " lane-change candidates or involved vehicles in one step");
+        if (error & 2) throw std::runtime_error("cityflow_b200: lane change ran out of spare slots for shadows");
+    }
     // First half of a step: ingest, segment index, signals, scheduling.  `spare` = free slots lent for this
-    // step's shadows.  Synchronises and returns the shadows created, in schedule order (= the order their
-    // priorities are drawn from the engine RNG, vehicle.cpp:33).
+    // step's shadows; the device takes them from the front.  Synchronises and returns the shadows created, in
+    // schedule order (= the order their priorities are drawn from the engine RNG, vehicle.cpp:33).  Throws when
+    // the step found more than LC_MAX_CANDIDATES candidates or used up the spares.
     void stepLcBegin(const SpawnRec *recs, int n, const int32_t *spare, int nSpare, std::vector<LcShadow> &created);
     // Second half: the drawn priorities, then leader pass, notify, control (+ sequential tail), move, leader.
     void stepLcEnd(const int32_t *priorities, int n);

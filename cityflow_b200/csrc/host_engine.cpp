@@ -109,6 +109,7 @@ public:
     std::vector<SpeedRec> replayRecs;
     std::vector<ReplayVehicle> replayVeh;
     std::vector<DeviceSim::LcDebugRec> replayRecsLc;
+    std::vector<int32_t> lcSpare;                            // slots lent to a lane-change step for its shadows
     std::vector<ReplayVehicleLc> replayVehLc;
     std::vector<int32_t> replayPhase;
     std::string replayLine;
@@ -705,8 +706,11 @@ public:
     }
     // One step with lane change: the shadows' priorities come from the engine RNG right after
     // this step's spawn draws (vehicle.cpp:33), so the step has a host round trip in the middle.
+    // The device is lent one spare slot per candidate it can schedule, so shadows never run out of slots and the
+    // candidate capacity is the only lane-change limit.
     void nextStepLaneChange() {
-        std::vector<int32_t> spare(256);
+        std::vector<int32_t> &spare = lcSpare;
+        spare.resize(DeviceSim::LC_MAX_CANDIDATES);
         for (auto &x : spare) { x = allocSlot(); slots[x].live = false; }
         prepareStep();                                   // (ensures device capacity for every slot handed out so far)
         for (const SpawnRec &r : batch)                  // the id's counter must leave room for the shadow suffixes

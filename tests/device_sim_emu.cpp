@@ -148,7 +148,7 @@ void DeviceSim::stepLcBegin(const SpawnRec *recs, int n, const int32_t *spare, i
             H.run(G, [&](int, int) { k_lc_schedule_roads(V, V.lc); });
             H.run(1, [&](int, int) { k_lc_log(V, V.lc); });
         }
-    if (H.lcCtrl.error) throw std::runtime_error("cityflow_b200: lane-change capacity exceeded (candidates per step or spare slots)");
+    lcCheckCapacity(H.lcCtrl.error);
     created.resize(H.lcCtrl.nShadows);
     for (int k = 0; k < H.lcCtrl.nShadows; ++k) created[k] = LcShadow{H.shadowLog[k].x, H.shadowLog[k].y};
     launches_ += 6;

@@ -24,6 +24,10 @@ priority-ordered build (oracle/lc_order_patch.sh), whose tie order is ascending 
 change drivable per step.  Flow intervals are at least 1 s (flow.h:34 asserts it).  The fixed-time plans hold the
 approaches red, not rlTrafficLight: the unmodified reference is run from the JSON alone.
 
+``replicated`` puts K disjoint copies of a small scenario (a dense 2x2 grid, or long_queue) into one roadnet, so that the
+per-step counts of lane change (candidates, involved vehicles, new shadows) grow K-fold while the restatement stays
+affordable.
+
 The ``reach`` helpers measure what a run actually reached, so that a test can assert its edge."""
 import math
 import random
@@ -332,6 +336,156 @@ def write(shape: str, directory: str, seed: int = 1, lane_change: bool = False) 
     net, flows = make(seed)
     return scenario.write_scenario(directory, net, flows, interval=interval, seed=seed, lane_change=lane_change,
                                    name="%s%d%s" % (shape, seed, "_lc" if lane_change else ""))
+
+
+def _grid2x2_unit(seed):
+    """A dense 2x2 grid: every road with a successor starts a flow, one vehicle every 2 s."""
+    from cityflow_b200 import scenario
+    net = scenario.grid_roadnet(2, 2)
+    return net, scenario.random_walk_flows(net, frac=1.0, interval=2.0, seed=seed)
+
+
+# unit: (roadnet and flows of a seed, default seed, step interval)
+REPLICA_UNITS = {"grid2x2": (_grid2x2_unit, 3, 1.0), "long_queue": (long_queue, 1, 1.0)}
+
+
+def replicated(unit: str, k: int, seed=None, dx: float = 5000.0):
+    """(roadnet, flows): `k` disjoint copies of `unit`, copy c prefixed "c<c>_" in every intersection, road and route id
+    and moved by c * dx along x (every point: roads, intersections, laneLinks).  Nothing joins two copies, so a run
+    carries k independent scenarios and its per-step counts (vehicles, lane-change candidates, shadows) grow k-fold."""
+    import copy
+    make, default_seed, _ = REPLICA_UNITS[unit]
+    net, flows = make(default_seed if seed is None else seed)
+
+    def moved(p, c):
+        return {**p, "x": p["x"] + c * dx}
+
+    out_net, out_flows = {"intersections": [], "roads": []}, []
+    for c in range(k):
+        pre = "c%d_" % c
+        for inter in net["intersections"]:
+            i = copy.deepcopy(inter)
+            i["id"] = pre + i["id"]
+            i["point"] = moved(i["point"], c)
+            i["roads"] = [pre + r for r in i["roads"]]
+            for rl in i["roadLinks"]:
+                rl["startRoad"], rl["endRoad"] = pre + rl["startRoad"], pre + rl["endRoad"]
+                for ll in rl["laneLinks"]:
+                    if "points" in ll:
+                        ll["points"] = [moved(p, c) for p in ll["points"]]
+            out_net["intersections"].append(i)
+        for road in net["roads"]:
+            r = copy.deepcopy(road)
+            r["id"] = pre + r["id"]
+            r["startIntersection"], r["endIntersection"] = pre + r["startIntersection"], pre + r["endIntersection"]
+            r["points"] = [moved(p, c) for p in r["points"]]
+            out_net["roads"].append(r)
+        for f in flows:
+            g = copy.deepcopy(f)
+            g["route"] = [pre + r for r in g["route"]]
+            out_flows.append(g)
+    return out_net, out_flows
+
+
+def write_replicated(directory: str, k: int, unit: str = "grid2x2", lane_change: bool = True, seed=None, dx: float = 5000.0) -> str:
+    """The config of `k` disjoint copies of `unit` (see replicated) in `directory`, at the unit's step interval."""
+    from cityflow_b200 import scenario
+    net, flows = replicated(unit, k, seed, dx)
+    s = REPLICA_UNITS[unit][1] if seed is None else seed
+    return scenario.write_scenario(directory, net, flows, interval=REPLICA_UNITS[unit][2], seed=s, lane_change=lane_change,
+                                   name="%s_x%d%s" % (unit, k, "_lc" if lane_change else ""))
+
+
+def device_form_restatement(cfg: str):
+    """The restatement (oracle.harness.PortOracle) in the decomposition the device runs (cfo_set_device_form): bit-equal
+    to the default form, and it counts the sizes of the lane-change step's sequential parts (cfo_device_form_stats)."""
+    import ctypes
+    from oracle import harness as H
+    o = H.PortOracle(cfg)
+    o.lib.cfo_set_device_form.restype = None
+    o.lib.cfo_set_device_form.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    o.lib.cfo_set_device_form(o.h, 1)
+    return o
+
+
+def lc_records(eng):
+    """cfb_debug_lc_vehicles of a CEngine: every running vehicle, shadows included, as oracle.harness.LC_DTYPE records in
+    ascending priority.  Identities are priorities, never slots."""
+    import ctypes
+    from oracle import harness as H
+    lib = eng.lib
+    lib.cfb_debug_lc_vehicles.restype = ctypes.c_int64
+    lib.cfb_debug_lc_vehicles.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64]
+    n = int(lib.cfb_debug_lc_vehicles(eng.h, None, 0))
+    got = np.zeros(n, H.LC_DTYPE)
+    if n:
+        lib.cfb_debug_lc_vehicles(eng.h, got.ctypes.data, n)
+    return got
+
+
+class LcReach:
+    """What a lane-change run reached, from the device-form restatement (device_form_restatement): the most candidates
+    (vehicles asking to change lanes) and involved vehicles (caught up in a change) in one step, the most candidates on
+    one road, and the most shadows created in one step (shadow priorities the step before did not have)."""
+
+    def __init__(self, ora):
+        import ctypes
+        self.ora = ora
+        ora.lib.cfo_device_form_stats.restype = None
+        ora.lib.cfo_device_form_stats.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        self.new_shadows = self.shadow_states = self.steps = self.max_vehicles = 0
+        self.prev = set()
+
+    def add(self, records):
+        sh = set(records["priority"][records["partner_type"] == 2].tolist())
+        self.new_shadows = max(self.new_shadows, len(sh - self.prev))
+        self.shadow_states += len(sh)
+        self.max_vehicles = max(self.max_vehicles, len(records))
+        self.prev = sh
+        self.steps += 1
+
+    def stats(self):
+        import ctypes
+        out = (ctypes.c_double * 6)()
+        self.ora.lib.cfo_device_form_stats(self.ora.h, out)
+        return dict(candidates=int(out[1]), candidates_on_a_road=int(out[2]), involved=int(out[4]))
+
+    def __str__(self):
+        s = self.stats()
+        return ("%d steps, up to %d running vehicles: at most %d candidates (%d on one road), %d involved vehicles and %d new "
+                "shadows in one step; %d shadow states" % (self.steps, self.max_vehicles, s["candidates"], s["candidates_on_a_road"],
+                                                         s["involved"], self.new_shadows, self.shadow_states))
+
+
+def lc_vs_restatement(engines: dict, cfg: str, steps: int) -> LcReach:
+    """Step the lane-change engines of `engines` (name -> CEngine or its emulated-device form) and the device-form
+    restatement together.  After every step, each engine's vehicle count, lane counts and records (lc_records: every
+    field, shadows included, keyed by priority) must equal the restatement's.  Returns what the run reached."""
+    import ctypes
+    from oracle import harness as H
+    ora = device_form_restatement(cfg)
+    reach = LcReach(ora)
+    lib = ora.lib
+    lib.cfo_lc_vehicles.restype = ctypes.c_int
+    lib.cfo_lc_vehicles.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
+    for s in range(1, steps + 1):
+        for eng in engines.values():
+            eng.next_step()
+        ora.next_step()
+        want = np.zeros(lib.cfo_lc_vehicles(ora.h, None, 0), H.LC_DTYPE)   # lc_snapshot's records, without the list orders
+        lib.cfo_lc_vehicles(ora.h, want.ctypes.data, len(want))
+        count, lanes = ora.vehicle_count(), ora.lane_vehicle_count()
+        reach.add(want)
+        for name, eng in engines.items():
+            got = lc_records(eng)
+            assert eng.vehicle_count() == count, "%s, step %d" % (name, s)
+            assert np.array_equal(eng.lane_vehicle_count(), lanes), "%s, lane counts, step %d" % (name, s)
+            assert len(got) == len(want), "%s, step %d: %d records, restatement %d" % (name, s, len(got), len(want))
+            for f in H.LC_DTYPE.names:
+                bad = np.nonzero(got[f] != want[f])[0]
+                assert not len(bad), "%s, step %d, field %s differs for %d vehicles, first priority %d: %r, restatement %r" % (
+                    name, s, f, len(bad), want["priority"][bad[0]], got[f][bad[0]], want[f][bad[0]])
+    return reach
 
 
 def write_spawn_burst(directory: str, n_flows: int = 2200) -> str:
